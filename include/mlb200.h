@@ -349,7 +349,7 @@ void mlb_interpolate_coeffs_linear(const float* c0, const float* c1, int n_coeff
 
 /* ---- device / context ---- */
 /* One device per process (the multi-GPU model is one process per GPU): mlb_init(other) while graphs, voice
- * banks or resamplers of the current device are alive returns MLB_ERR_INVALID.  Entry points make the
+ * banks, resamplers or FDTD banks of the current device are alive returns MLB_ERR_INVALID.  Entry points make the
  * library's device current on the calling thread. */
 int mlb_init(int device);          /* select device, check sm_90; MLB_ERR_NO_DEVICE if absent */
 int mlb_device_count(void);        /* 0 when no GPU: callers must fail loudly, not fall back */
@@ -374,6 +374,28 @@ int mlb_resampler_process_host(mlb_resampler* r, const float* in_host, float* ou
                                int* n_blocks_out);
 int mlb_resampler_process_device(mlb_resampler* r, const float* in_dev, float* out_dev, int n_blocks_in,
                                  int* n_blocks_out, void* stream);
+
+/* ---- FDTD membrane banks (K9) ---------------------------------------------------------------
+ * V independent 16 x 16 finite-difference membranes = V x (FDTDState + processFDTDModel) of the reference's
+ * examples/audio-and-midi/fdtd.cpp:26-154: per sample, the coefficients are designed from the frequency
+ * sample (cycles per sample), the excitation sample times 4 is added to the z^-1 surface at row 2, column 8,
+ * one explicit step of the 3 x 3 stencil over the z^-1 and z^-2 surfaces gives the new surface (fixed zero
+ * boundary), and its cells at row 9, columns 1 and 15 are the L and R outputs.  Bit-exact: every op is one
+ * separately rounded binary32 op in the reference's order.  One kernel launch per call. */
+typedef struct mlb_fdtd mlb_fdtd;        /* V membranes = V FDTDState + processFDTDModel, fdtd.cpp:26-154 */
+#define MLB_FDTD_SIZE 16                 /* kWidth = kHeight */
+#define MLB_FDTD_FTZ 1u                  /* every FP op flushes subnormals, as under UsingFlushDenormalsToZero */
+/* inputs are [T][in_planes][V][64]; rows excite_plane / freq_plane (cycles per sample) are read, so a graph's
+ * or a Voice bank's output buffer can be passed as-is.  State after create/clear: all surfaces zero. */
+int mlb_fdtd_create(int n_instances, float sample_rate, int in_planes, int excite_plane, int freq_plane,
+                    unsigned flags, mlb_fdtd** out);
+int mlb_fdtd_destroy(mlb_fdtd* f);
+int mlb_fdtd_clear(mlb_fdtd* f);
+int mlb_fdtd_get_state(mlb_fdtd* f, float* host);        /* [V][2][16][16]: z^-1 interior, then z^-2 */
+int mlb_fdtd_set_state(mlb_fdtd* f, const float* host);
+int mlb_fdtd_process_device(mlb_fdtd* f, const float* in_dev, float* out_dev /* [T][2][V][64] L,R */,
+                            int n_blocks, void* stream);
+int mlb_fdtd_process_host(mlb_fdtd* f, const float* in_host, float* out_host, int n_blocks);
 
 /* ---- EventsToSignals::Voice bank (SURVEY 8f row 3) ---------------------------------------
  * The step BEFORE the chain: the reference's EventsToSignals (source/app/MLEventsToSignals.h:43-236)

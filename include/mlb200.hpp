@@ -703,4 +703,37 @@ class Resampler
   }
 };
 
+// ---- FDTDBank: V x the FDTD membrane of examples/audio-and-midi/fdtd.cpp on the GPU (mlb_fdtd_*) ----
+// What FDTDState + processFDTDModel(input, freq, &state) is per instance.
+class FDTDBank
+{
+  mlb_fdtd* f_ = nullptr;
+  int n_ = 0, planes_ = 0;
+
+ public:
+  FDTDBank(int nInstances, float sampleRate = 48000.f, int inPlanes = 2, int excitePlane = 0, int freqPlane = 1,
+           unsigned flags = 0)
+      : n_(nInstances), planes_(inPlanes)
+  {
+    check(mlb_fdtd_create(nInstances, sampleRate, inPlanes, excitePlane, freqPlane, flags, &f_));
+  }
+  ~FDTDBank() { mlb_fdtd_destroy(f_); }
+  FDTDBank(const FDTDBank&) = delete;
+  FDTDBank& operator=(const FDTDBank&) = delete;
+  int instances() const { return n_; }
+  int inputPlanes() const { return planes_; }
+  mlb_fdtd* handle() const { return f_; }
+  void clear() { check(mlb_fdtd_clear(f_)); }
+  // [instances][2][16][16]: z^-1 surface, then z^-2
+  void getState(float* host) { check(mlb_fdtd_get_state(f_, host)); }
+  void setState(const float* host) { check(mlb_fdtd_set_state(f_, host)); }
+  // host buffers: in [nBlocks][inPlanes][instances][64] -> out [nBlocks][2][instances][64]
+  void process(const float* in, float* out, int nBlocks) { check(mlb_fdtd_process_host(f_, in, out, nBlocks)); }
+  // device buffers, asynchronous on `stream` (a cudaStream_t)
+  void processDevice(const float* in, float* out, int nBlocks, void* stream = nullptr)
+  {
+    check(mlb_fdtd_process_device(f_, in, out, nBlocks, stream));
+  }
+};
+
 }  // namespace mlb

@@ -90,7 +90,14 @@ def lib() -> ctypes.CDLL:
     L.mlb_resampler_clear.argtypes = [_vp]
     L.mlb_resampler_process_host.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp]
     L.mlb_resampler_process_device.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp, _vp]
-    L.mlb_voices_create.argtypes = [ctypes.c_int, _cf, _vp, _vp, _vp, _vp, ctypes.c_uint, _vp]
+    L.mlb_fdtd_create.argtypes = [ctypes.c_int, _cf, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_uint, _vp]
+    L.mlb_fdtd_destroy.argtypes = [_vp]
+    L.mlb_fdtd_clear.argtypes = [_vp]
+    L.mlb_fdtd_get_state.argtypes = [_vp, _vp]
+    L.mlb_fdtd_set_state.argtypes = [_vp, _vp]
+    L.mlb_fdtd_process_device.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp]
+    L.mlb_fdtd_process_host.argtypes = [_vp, _vp, _vp, ctypes.c_int]
+    L.mlb_voices_create.argtypes =[ctypes.c_int, _cf, _vp, _vp, _vp, _vp, ctypes.c_uint, _vp]
     L.mlb_voices_destroy.argtypes = [_vp]
     L.mlb_voices_set_main_voices.argtypes = [_vp, _vp]
     L.mlb_voices_process_host.argtypes = [_vp, _vp, _vp, ctypes.c_int, ctypes.c_uint]
@@ -522,6 +529,61 @@ class ResamplerBank:
         n = ctypes.c_int(0)
         _check(lib().mlb_resampler_process_host(self._h, x.ctypes.data, out.ctypes.data, T, ctypes.byref(n)))
         return out[:n.value]
+
+
+class FDTDBank:
+    """V x the reference's FDTD membrane (FDTDState + processFDTDModel, examples/audio-and-midi/fdtd.cpp): per
+    block, an excitation row and a frequency row (cycles per sample) in, the two pickup rows L, R out."""
+
+    FTZ = 1  # MLB_FDTD_FTZ: every FP op flushes subnormals, as under UsingFlushDenormalsToZero
+    SIZE = 16
+
+    def __init__(self, n_instances: int, sample_rate: float = 48000.0, in_planes: int = 2, excite_plane: int = 0,
+                 freq_plane: int = 1, flags: int = 0):
+        self.n_instances, self.in_planes = int(n_instances), int(in_planes)
+        h = ctypes.c_void_p()
+        _check(lib().mlb_fdtd_create(self.n_instances, sample_rate, self.in_planes, excite_plane, freq_plane, flags,
+                                     ctypes.byref(h)))
+        self._h = h
+
+    def close(self) -> None:
+        if self._h:
+            lib().mlb_fdtd_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def clear(self) -> None:
+        _check(lib().mlb_fdtd_clear(self._h))
+
+    def get_state(self) -> np.ndarray:
+        """[V][2][16][16]: the z^-1 surface, then z^-2."""
+        st = np.zeros((self.n_instances, 2, self.SIZE, self.SIZE), np.float32)
+        _check(lib().mlb_fdtd_get_state(self._h, st.ctypes.data))
+        return st
+
+    def set_state(self, state: np.ndarray) -> None:
+        st = np.ascontiguousarray(state, np.float32)
+        assert st.shape == (self.n_instances, 2, self.SIZE, self.SIZE), st.shape
+        _check(lib().mlb_fdtd_set_state(self._h, st.ctypes.data))
+
+    def process_host(self, inp: np.ndarray) -> np.ndarray:
+        """inp [T][in_planes][V][64] -> out [T][2][V][64] (pickups L, R)."""
+        inp = np.ascontiguousarray(inp, np.float32)
+        if inp.ndim != 4 or inp.shape[1:] != (self.in_planes, self.n_instances, BLOCK):
+            raise ValueError(f"process_host: inp must be [T][{self.in_planes}][{self.n_instances}][64], got {inp.shape}")
+        out = np.empty((inp.shape[0], 2, self.n_instances, BLOCK), np.float32)
+        _check(lib().mlb_fdtd_process_host(self._h, inp.ctypes.data, out.ctypes.data, inp.shape[0]))
+        return out
+
+    def process_device(self, inp, out, n_blocks: int, stream: int = 0) -> None:
+        """Device buffers (torch tensors / ints): inp [T][in_planes][V][64], out [T][2][V][64]; asynchronous on
+        ``stream``, one kernel launch, no allocation or synchronisation (capturable into a CUDA graph)."""
+        _check(lib().mlb_fdtd_process_device(self._h, _ptr(inp), _ptr(out), int(n_blocks), stream or None))
 
 
 class _Event(ctypes.Structure):

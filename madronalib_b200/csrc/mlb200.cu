@@ -24,6 +24,7 @@
 #include "fdn_kernel.cuh"
 #include "voice_kernel.cuh"
 #include "resample_kernel.cuh"
+#include "fdtd_kernel.cuh"
 #include "generic_kernel.cuh"
 
 using namespace mlb;
@@ -419,7 +420,7 @@ extern "C" void mlb_coeffs_fdn8(const float times[8], const float cutoffs[8], co
 // device
 
 static int g_device = -1;
-static std::atomic<int> g_live_handles{0};  // graphs + voice banks + resamplers alive (they hold pointers of g_device)
+static std::atomic<int> g_live_handles{0};  // graphs + voice banks + resamplers + FDTD banks alive (they hold pointers of g_device)
 static int g_sm_count = 0;
 static size_t g_smem_optin = 0;
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
@@ -2668,6 +2669,129 @@ extern "C" int mlb_resampler_process_host(mlb_resampler* r, const float* in_host
   rc = mlb_resampler_process_device(r, r->d_in, r->d_out, n_blocks_in, n_blocks_out, s);
   if (rc != MLB_OK) return rc;
   if (n_out > 0) CU_CHECK(cudaMemcpyAsync(out_host, r->d_out, (size_t)n_out * row, cudaMemcpyDeviceToHost, s));
+  CU_CHECK(cudaStreamSynchronize(s));
+  return MLB_OK;
+}
+
+// ------------------------------------------------------------------------------------------
+// FDTD membrane banks (K9, fdtd_kernel.cuh)
+
+struct mlb_fdtd
+{
+  int V = 0, in_planes = 0, excite = 0, freq = 0;
+  unsigned flags = 0;
+  float sample_rate = 0.f;
+  float* d_state = nullptr;  // [V][2][16][16]
+  float *d_in = nullptr, *d_out = nullptr;
+  size_t in_cap = 0, out_cap = 0;
+  cudaStream_t stream = nullptr;
+};
+
+static size_t fdtd_state_bytes(const mlb_fdtd* f) { return (size_t)f->V * 2 * kFdtdCells * sizeof(float); }
+
+extern "C" int mlb_fdtd_destroy(mlb_fdtd* f)
+{
+  if (!f) return MLB_OK;
+  cudaFree(f->d_state);
+  cudaFree(f->d_in);
+  cudaFree(f->d_out);
+  if (f->stream) cudaStreamDestroy(f->stream);
+  delete f;
+  --g_live_handles;
+  return MLB_OK;
+}
+extern "C" int mlb_fdtd_clear(mlb_fdtd* f)
+{
+  if (!f) return fail(MLB_ERR_INVALID, "null FDTD bank");
+  CU_CHECK(cudaMemset(f->d_state, 0, fdtd_state_bytes(f)));
+  CU_CHECK(cudaDeviceSynchronize());
+  return MLB_OK;
+}
+extern "C" int mlb_fdtd_create(int n_instances, float sample_rate, int in_planes, int excite_plane, int freq_plane,
+                               unsigned flags, mlb_fdtd** out)
+{
+  if (!out) return fail(MLB_ERR_INVALID, "out is null");
+  *out = nullptr;
+  if (n_instances <= 0) return fail(MLB_ERR_INVALID, "n_instances must be positive (got %d)", n_instances);
+  if (!(sample_rate > 0.f) || !std::isfinite(sample_rate))
+    return fail(MLB_ERR_INVALID, "sample_rate must be positive and finite (got %g)", (double)sample_rate);
+  if (in_planes <= 0 || excite_plane < 0 || excite_plane >= in_planes || freq_plane < 0 || freq_plane >= in_planes)
+    return fail(MLB_ERR_INVALID, "bad planes (in_planes %d, excite_plane %d, freq_plane %d)", in_planes,
+                excite_plane, freq_plane);
+  if (flags & ~MLB_FDTD_FTZ) return fail(MLB_ERR_INVALID, "unknown flags 0x%x", flags);
+  int rc = ensure_init();
+  if (rc != MLB_OK) return rc;
+  mlb_fdtd* f = new mlb_fdtd;
+  ++g_live_handles;
+  f->V = n_instances, f->in_planes = in_planes, f->excite = excite_plane, f->freq = freq_plane;
+  f->flags = flags, f->sample_rate = sample_rate;
+  if (cudaMalloc(&f->d_state, fdtd_state_bytes(f)) != cudaSuccess)
+  {
+    mlb_fdtd_destroy(f);
+    return fail(MLB_ERR_ALLOC, "cudaMalloc of FDTD state failed");
+  }
+  cudaStreamCreateWithFlags(&f->stream, cudaStreamNonBlocking);
+  rc = mlb_fdtd_clear(f);
+  if (rc != MLB_OK)
+  {
+    mlb_fdtd_destroy(f);
+    return rc;
+  }
+  *out = f;
+  return MLB_OK;
+}
+extern "C" int mlb_fdtd_get_state(mlb_fdtd* f, float* host)
+{
+  if (!f || !host) return fail(MLB_ERR_INVALID, "null argument");
+  CU_CHECK(cudaDeviceSynchronize());
+  CU_CHECK(cudaMemcpy(host, f->d_state, fdtd_state_bytes(f), cudaMemcpyDeviceToHost));
+  return MLB_OK;
+}
+extern "C" int mlb_fdtd_set_state(mlb_fdtd* f, const float* host)
+{
+  if (!f || !host) return fail(MLB_ERR_INVALID, "null argument");
+  CU_CHECK(cudaDeviceSynchronize());
+  CU_CHECK(cudaMemcpy(f->d_state, host, fdtd_state_bytes(f), cudaMemcpyHostToDevice));
+  return MLB_OK;
+}
+extern "C" int mlb_fdtd_process_device(mlb_fdtd* f, const float* in_dev, float* out_dev, int n_blocks, void* stream)
+{
+  if (!f || !in_dev || !out_dev) return fail(MLB_ERR_INVALID, "null argument");
+  if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive (got %d)", n_blocks);
+  FdtdArgs a;
+  a.in = in_dev, a.out = out_dev, a.state = f->d_state;
+  a.V = f->V, a.T = n_blocks, a.in_planes = f->in_planes, a.excite_plane = f->excite, a.freq_plane = f->freq;
+  // the example's constants (fdtd.cpp:23, 79, 89, 100-101, 118), rounded on the host as its compiler does
+  a.k_size = sqrtf((float)(kFdtdN * kFdtdN) + (float)(kFdtdN * kFdtdN));
+  a.k_tension = 3.0f / 5.0f;
+  a.k_sixth = 1.f / 6.f;
+  a.k_two_thirds = 2.f / 3.f;
+  a.isr = 1.0f / f->sample_rate;
+  a.sk = 1.0f / (1.0f + a.isr * 1.0f);
+  const int grid = (f->V + kFdtdWarps - 1) / kFdtdWarps;
+  if (f->flags & MLB_FDTD_FTZ)
+    fdtd_kernel<true><<<grid, 32 * kFdtdWarps, 0, (cudaStream_t)stream>>>(a);
+  else
+    fdtd_kernel<false><<<grid, 32 * kFdtdWarps, 0, (cudaStream_t)stream>>>(a);
+  ++g_launches;
+  CU_CHECK(cudaGetLastError());
+  return MLB_OK;
+}
+extern "C" int mlb_fdtd_process_host(mlb_fdtd* f, const float* in_host, float* out_host, int n_blocks)
+{
+  if (!f || !in_host || !out_host) return fail(MLB_ERR_INVALID, "null argument");
+  if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive (got %d)", n_blocks);
+  const size_t row = (size_t)f->V * MLB_BLOCK * sizeof(float);
+  const size_t in_bytes = (size_t)n_blocks * f->in_planes * row, out_bytes = (size_t)n_blocks * 2 * row;
+  int rc = ensure_buf(&f->d_in, &f->in_cap, in_bytes);
+  if (rc != MLB_OK) return rc;
+  rc = ensure_buf(&f->d_out, &f->out_cap, out_bytes);
+  if (rc != MLB_OK) return rc;
+  cudaStream_t s = f->stream;
+  CU_CHECK(cudaMemcpyAsync(f->d_in, in_host, in_bytes, cudaMemcpyHostToDevice, s));
+  rc = mlb_fdtd_process_device(f, f->d_in, f->d_out, n_blocks, s);
+  if (rc != MLB_OK) return rc;
+  CU_CHECK(cudaMemcpyAsync(out_host, f->d_out, out_bytes, cudaMemcpyDeviceToHost, s));
   CU_CHECK(cudaStreamSynchronize(s));
   return MLB_OK;
 }

@@ -809,3 +809,52 @@ def random_graph_workload(seed: int, n_voices: int = 37, n_nodes: int = 24, hw_a
         return np.concatenate([(x * gate).astype(np.float32), ctl * np.float32(60.0)], axis=1)
     w.inputs = _rows_inputs(fn)  # type: ignore[assignment]
     return w
+
+
+# ---- K9: the FDTD membrane of examples/audio-and-midi/fdtd.cpp ----
+
+def fdtd_example(n_instances: int) -> Workload:
+    """The first lines of the example's processFDTD (fdtd.cpp:165-170) as a graph, per instance:
+        ticks = ImpulseGen(2/sr) * 0.1;  freq = (220 + SineGen(0.15/sr) * 40) / sr   (sr = 48000)
+    with freshly constructed generators.  Outputs [ticks, freq]: the graph's [T][2][V][64] output buffer is the
+    input of an FDTDBank(V, in_planes=2, excite_plane=0, freq_plane=1, flags=FTZ) as it stands."""
+    V = n_instances
+    g = GraphSpec()
+    f_imp, gain, f_sin, depth, center, rate = (g.param() for _ in range(6))
+    ticks = g.node("MULTIPLY", g.node("IMPULSE", f_imp), gain)
+    freq = g.node("DIVIDE", g.node("ADD", center, g.node("MULTIPLY", g.node("SINE", f_sin), depth)), rate)
+    g.output(ticks, freq)
+    coef, state = g.new_coefs(V), g.new_state(V)
+    sr = np.float32(SR)
+    for node, value in ((f_imp, np.float32(2.0) / sr), (gain, np.float32(0.1)), (f_sin, np.float32(0.15) / sr),
+                        (depth, np.float32(40.0)), (center, np.float32(220.0)), (rate, sr)):
+        coef[g.coef_slot(node)] = value
+    return Workload("fdtd_example", g, V, coef, state)
+
+
+FDTD_BURST_PERIOD = 375  # vectors between two excitations of one membrane (the example's impulse rate at 48 kHz)
+
+
+def fdtd_inputs(n_instances: int, n_blocks: int, t0: int = 0, v0: int = 0, v1: Optional[int] = None) -> np.ndarray:
+    """Excitation and frequency rows for a bank of FDTD membranes, [T][2][V'][64] f32 for instances [v0, v1):
+      excitation: one vector of noise (uniform in +-0.1, a seeded function of instance and vector) every
+                  FDTD_BURST_PERIOD vectors, instance v firing at vectors t = (53 v) mod FDTD_BURST_PERIOD + k P;
+      frequency:  Fs_v[n] = (100 + 900 v / V) / 48000 * (1 + 0.1 tri(((n + 97 v) mod 4800) / 4800)) cycles per sample,
+                  n = absolute sample index, tri = 0..1..0 -- at most 0.0229, inside the stable range (T^2 < 3/5,
+                  i.e. Fs below ~0.057)."""
+    V = n_instances
+    v1 = V if v1 is None else v1
+    vv = np.arange(v0, v1, dtype=np.int64)
+    out = np.zeros((n_blocks, 2, v1 - v0, BLOCK), np.float32)
+    base = ((np.float32(100.0) + np.float32(900.0) * vv.astype(np.float32) / np.float32(V)) / np.float32(SR))[:, None]
+    for t in range(n_blocks):
+        ta = t0 + t
+        fire = np.nonzero((ta - 53 * vv) % FDTD_BURST_PERIOD == 0)[0]
+        for i in fire:
+            rng = np.random.default_rng((int(vv[i]) << 20) ^ ta)
+            out[t, 0, i] = rng.uniform(-0.1, 0.1, BLOCK).astype(np.float32)
+        n = np.arange(BLOCK, dtype=np.int64)[None, :] + ta * BLOCK + 97 * vv[:, None]
+        ph = (n % 4800).astype(np.float32) / np.float32(4800.0)
+        tri = np.float32(1.0) - np.abs(np.float32(2.0) * ph - np.float32(1.0))
+        out[t, 1] = base * (np.float32(1.0) + np.float32(0.1) * tri)
+    return out

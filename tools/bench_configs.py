@@ -2,11 +2,13 @@
 """Kernel-resident timing of everything except the headline: BASELINE.json configurations 2-5, the
 SURVEY 8(f) workloads (config 6 = Aaltoverb x V, the EventsToSignals::Voice bank) and the elementwise maps.
 
-    python tools/bench_configs.py [--steps K] [--only 2,3,4,5,6,voices,map] [--generic] [--cpu]
+    python tools/bench_configs.py [--steps K] [--only 2,3,4,5,6,voices,map,fdtd] [--generic] [--cpu]
 
 Prints one JSON line per configuration: kernel name, mean CUDA-event kernel time, algorithmic
 bytes per launch (SURVEY.md 8d / DESIGN.md), achieved GB/s and fraction of the measured HBM peak.
---cpu also times the reference (oracle/_ref) on the box's host cores for config 6 and the Voice bank.
+--cpu also times the reference (oracle/_ref) on the box's host cores for config 6, the Voice bank and the FDTD
+membranes.  The FDTD lines (K9) are compute-bound: they report instance-samples/s and the share of the FP32 issue
+ceiling instead of bytes.
 Not the headline benchmark (that is bench.py / config A).
 """
 import argparse
@@ -26,10 +28,11 @@ def main():
     from madronalib_b200 import api, workloads as wl
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
-    ap.add_argument("--only", default="2,3,swept,4,5,6,voices,map")
+    ap.add_argument("--only", default="2,3,swept,4,5,6,voices,map,fdtd")
     ap.add_argument("--generic", action="store_true", help="force the graph interpreter kernel")
     ap.add_argument("--cpu", action="store_true",
-                    help="also time the reference (oracle/_ref, all host threads) on config 6 and the Voice bank")
+                    help="also time the reference (oracle/_ref, all host threads) on config 6, the Voice bank "
+                         "and the FDTD membranes")
     args = ap.parse_args()
     only = set(args.only.split(","))
     api.init(0)
@@ -112,6 +115,8 @@ def main():
                               "frac_of_measured_hbm_peak": b / (ms * 1e-3) / 1e9 / peak}), flush=True)
             vb.close()
         del d_ev, d_rows
+    if "fdtd" in only:
+        bench_fdtd(api, wl, torch, dev, args.steps, args.cpu)
     if args.cpu:
         # the reference itself on this box's host cores (oracle/_ref; checker code, used here only as a baseline)
         import time
@@ -162,6 +167,104 @@ def main():
                           "frac_of_measured_hbm_peak": b / (kms * 1e-3) / 1e9 / peak,
                           "delay_memory_mb": g.delay_bytes / 1e6}), flush=True)
         g.close()
+        del d_in, d_out
+
+
+# K9's arithmetic, counted from the example's text (fdtd.cpp:85-129 and doFDTDStep2D :64-69) rather than typed in:
+# the stencil is a sum of terms coefficient * (sum of n cells); the coefficient design and the exciter are
+# lists of (multiplies, adds) per step.
+FDTD_STENCIL_TERMS = (("kc", 1), ("ke", 4), ("kk", 4), ("kc2", 1), ("ke2", 4))
+FDTD_DESIGN_STEPS = (("c = kSize Fs", 1, 0), ("T = 3/5 c", 1, 0), ("T T", 1, 0), ("kk", 1, 0), ("ke", 1, 0),
+                     ("kc = 2 - 4 (kk + ke)", 1, 2), ("ks1 = s1 T isr", 2, 0), ("ke += ks1", 0, 1),
+                     ("kc += -4 ks1", 1, 1), ("ke2 = -1 ks1", 1, 0), ("kc2 = s0 isr + 4 ks1 - 1", 2, 2),
+                     ("5 x *= SK", 5, 0), ("exciter += in kInputGain", 1, 1))
+
+
+def fdtd_ops_per_sample():
+    """(stencil ops per cell, design + exciter ops per sample, total FP32 ops per instance-sample)."""
+    cell = sum(1 + (n - 1) for _, n in FDTD_STENCIL_TERMS) + (len(FDTD_STENCIL_TERMS) - 1)
+    design = sum(m + a for _, m, a in FDTD_DESIGN_STEPS)
+    return cell, design, 16 * 16 * cell + design
+
+
+def gpu_facts():
+    """Card name, power limit (W) and SM clocks (MHz, current and maximum), read in this run (read-only query)."""
+    import subprocess
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm",
+                            "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=30)
+        name, pl, sm, smax = [x.strip() for x in r.stdout.strip().split("\n")[0].split(",")]
+        return {"gpu": name, "power_limit_w": float(pl), "sm_clock_mhz": float(sm), "sm_clock_max_mhz": float(smax)}
+    except Exception as e:  # noqa: BLE001
+        return {"gpu": "unknown (%s)" % e}
+
+
+def bench_fdtd(api, wl, torch, dev, steps, cpu):
+    """K9: V FDTD membranes x 64 vectors, inputs resident on the device, both floating-point modes.  Mean of `steps`
+    CUDA-event-timed launches after 3 warm-up launches; parity of 64 instances of the last timed launch against the
+    checker (the example's text where oracle/_ref was built, else the plain-C port)."""
+    from oracle import fdtd_bindings as ob
+    T = 64
+    cell, design, ops = fdtd_ops_per_sample()
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    for V in (4096, 16384):
+        inp = wl.fdtd_inputs(V, T)
+        d_in = torch.from_numpy(inp).to(dev)
+        d_out = torch.empty((T, 2, V, 64), dtype=torch.float32, device=dev)
+        sample = np.linspace(0, V - 1, 64).astype(np.int64)
+        for ftz in (False, True):
+            b = api.FDTDBank(V, 48000.0, flags=api.FDTDBank.FTZ if ftz else 0)
+            sh = torch.cuda.current_stream().cuda_stream
+            for _ in range(3):
+                b.process_device(d_in, d_out, T, sh)
+            times = []
+            for i in range(steps):
+                if i == steps - 1:
+                    torch.cuda.synchronize()
+                    st_before = b.get_state()[sample]
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                b.process_device(d_in, d_out, T, sh)
+                e1.record()
+                torch.cuda.synchronize()
+                times.append(e0.elapsed_time(e1))
+            facts = gpu_facts()
+            got = d_out[:, :, torch.from_numpy(sample).to(dev)].cpu().numpy()
+            sub_in = np.ascontiguousarray(inp[:, :, sample])
+            if ob.fdtd_ref_available():
+                want, _, _ = ob.RefFdtd().run(sub_in, st_before, ftz=ftz)
+                checker = "reference example text (oracle/_ref/libmlfdtd.so)"
+            else:
+                want, _ = ob.port_fdtd(sub_in, st_before, ftz=ftz)
+                checker = "plain-C port"
+            both_nan = np.isnan(got) & np.isnan(want)
+            mism = int(((got.view(np.uint32) != want.view(np.uint32)) & ~both_nan).sum())
+            b.close()
+            ms = float(np.mean(times))
+            rate = V * T * 64 / (ms * 1e-3)
+            clock = facts.get("sm_clock_max_mhz")
+            ceiling = sms * 128 * clock * 1e6 if clock else None
+            print(json.dumps({
+                "config": "fdtd_" + ("ftz" if ftz else "ieee"), "kernel": "fdtd_kernel<%s>" % ("true" if ftz else "false"),
+                "instances": V, "blocks": T, "kernel_ms": ms, "instance_samples_per_s": rate,
+                "membranes_realtime_48k": rate / 48000.0,
+                "fp32_ops_per_instance_sample": ops, "stencil_ops_per_cell": cell, "design_ops_per_sample": design,
+                "achieved_fp32_ops_per_s": rate * ops,
+                "non_fma_fp32_ceiling_ops_per_s": ceiling,
+                "frac_of_non_fma_ceiling": rate * ops / ceiling if ceiling else None,
+                "ceiling_note": "%d SMs x 128 FP32 lanes x max SM clock, one op per lane per clock: exact mode "
+                                "cannot fuse multiplies and adds, so the FMA data-sheet figure does not apply" % sms,
+                **facts, "parity_instances": 64, "parity_checker": checker, "mismatches": mism}), flush=True)
+        if cpu and ob.fdtd_ref_available():
+            cores = os.cpu_count() or 1
+            best = 1e30
+            for _ in range(2):
+                _, _, sec = ob.RefFdtd().run(inp, ftz=True, nthreads=cores)
+                best = min(best, sec)
+            print(json.dumps({"config": "fdtd_reference_cpu", "threads": cores, "instances": V, "blocks": T,
+                              "seconds": best, "instance_samples_per_s": V * T * 64 / best,
+                              "note": "the example's own processFDTDModel under UsingFlushDenormalsToZero "
+                                      "(oracle/_ref/libmlfdtd.so), same inputs"}), flush=True)
         del d_in, d_out
 
 
