@@ -349,7 +349,7 @@ void mlb_interpolate_coeffs_linear(const float* c0, const float* c1, int n_coeff
 
 /* ---- device / context ---- */
 /* One device per process (the multi-GPU model is one process per GPU): mlb_init(other) while graphs, voice
- * banks, resamplers or FDTD banks of the current device are alive returns MLB_ERR_INVALID.  Entry points make the
+ * banks, resamplers, FDTD banks or bus layouts of the current device are alive returns MLB_ERR_INVALID.  Entry points make the
  * library's device current on the calling thread. */
 int mlb_init(int device);          /* select device, check sm_90; MLB_ERR_NO_DEVICE if absent */
 int mlb_device_count(void);        /* 0 when no GPU: callers must fail loudly, not fall back */
@@ -605,6 +605,28 @@ int mlb_graph_plan(const mlb_node* nodes, int n_nodes, const int32_t* outs, int 
  * MLB_ERR_INVALID when the bank and the graph differ in voice count or the graph reads no Voice row. */
 int mlb_synth_process_host(mlb_voices* vb, mlb_graph* g, const mlb_voice_events* events_host,
                            float* out_host, float* mix_host, int n_blocks);
+
+/* ---- Per-instrument output buses (K10) ---------------------------------------------------------
+ * A reference Synth owns at most 16 voices (EventsToSignals::kMaxVoices, MLEventsToSignals.h:47), so a bank of V
+ * voices is in practice many instruments.  A bus layout is G voice ranges [first[g], first[g] + count[g]): a count
+ * of 0 gives a bus of +0; ranges may leave gaps (MPE: Synth reads getInputVoice(v) = voices[v + 1], so an
+ * instrument's main voice is not summed) and may overlap.  For every block t, plane p, bus g and sample n:
+ *   bus[t][p][g][n] = ((+0 + x[first]) + x[first + 1]) + ... + x[first + count - 1]
+ * one binary32 add per voice in voice order, subnormals kept: Synth::processVector (MLSynth.h:36-60) with the
+ * default isVoiceActive, bit for bit.  The bus rows [T][P][G][64] have the layout of a G-voice graph's input. */
+typedef struct mlb_buses mlb_buses;   /* G per-instrument output buses over a V-voice bank (Synth::processVector, MLSynth.h:36-60) */
+/* Validates the layout on the host (MLB_ERR_INVALID names the offending bus) and uploads it.  A live layout counts
+ * toward mlb_init's one-device rule. */
+int mlb_buses_create(int n_voices, int n_buses, const int32_t* first_voice, const int32_t* voice_count, mlb_buses** out);
+int mlb_buses_destroy(mlb_buses* b);
+/* rows_dev [T][n_planes][V][64] -> bus_dev [T][n_planes][G][64]; one launch, no allocation, no synchronisation */
+int mlb_buses_sum_device(mlb_buses* b, const float* rows_dev, float* bus_dev, int n_planes, int n_blocks, void* stream);
+/* contract E with per-instrument output: event records in, bus rows [T][n_out][G][64] out; voice rows never leave HBM.
+ * The pipeline of mlb_synth_process_host; the graph's rows of one time chunk go to a device scratch of one chunk
+ * and are summed into buses on the graph's stream right after the graph.  MLB_ERR_INVALID when the bank, graph and
+ * buses differ in voice count, the graph has no outputs or reads no Voice row. */
+int mlb_synth_process_buses_host(mlb_voices* vb, mlb_graph* g, mlb_buses* b, const mlb_voice_events* events_host,
+                                 float* bus_host, int n_blocks);
 
 #ifdef __cplusplus
 }

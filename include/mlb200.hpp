@@ -683,6 +683,41 @@ inline void processEvents(VoiceBank& voices, DeviceBank& bank, const mlb_voice_e
   check(mlb_synth_process_host(voices.handle(), bank.handle(), events, out, mix, nBlocks));
 }
 
+// ---- Buses: per-instrument output buses over a voice bank on the GPU (mlb_buses_*) ----
+// What one Synth::processVector (MLSynth.h:36-60) does per instrument: bus g = the strict left-to-right sum of the
+// voice rows [first[g], first[g] + count[g]), starting from +0.
+class Buses
+{
+  mlb_buses* b_ = nullptr;
+  int voices_ = 0, n_ = 0;
+
+ public:
+  Buses(int nVoices, int nBuses, const int32_t* firstVoice, const int32_t* voiceCount)
+      : voices_(nVoices), n_(nBuses)
+  {
+    check(mlb_buses_create(nVoices, nBuses, firstVoice, voiceCount, &b_));
+  }
+  ~Buses() { mlb_buses_destroy(b_); }
+  Buses(const Buses&) = delete;
+  Buses& operator=(const Buses&) = delete;
+  int voices() const { return voices_; }
+  int buses() const { return n_; }
+  mlb_buses* handle() const { return b_; }
+  // device buffers, asynchronous on `stream`: rows [nBlocks][nPlanes][voices][64] -> bus [nBlocks][nPlanes][buses][64]
+  void sumDevice(const float* rows, float* bus, int nPlanes, int nBlocks, void* stream = nullptr)
+  {
+    check(mlb_buses_sum_device(b_, rows, bus, nPlanes, nBlocks, stream));
+  }
+};
+
+// processEvents with per-instrument output (mlb_synth_process_buses_host): events [nBlocks][voices] in,
+// bus [nBlocks][n_out][buses][64] out; the voice rows stay on the device.
+inline void processEventsToBuses(VoiceBank& voices, DeviceBank& bank, Buses& buses, const mlb_voice_events* events,
+                                 float* bus, int nBlocks)
+{
+  check(mlb_synth_process_buses_host(voices.handle(), bank.handle(), buses.handle(), events, bus, nBlocks));
+}
+
 // ---- Resampler: Upsampler(octaves) / Downsampler(octaves) x V on the GPU (mlb_resampler_*) ----
 class Resampler
 {

@@ -104,6 +104,10 @@ def lib() -> ctypes.CDLL:
     L.mlb_voices_process_device.argtypes = [_vp, _vp, _vp, ctypes.c_int, ctypes.c_uint, _vp]
     L.mlb_graph_process_device.argtypes = [_vp, _vp, _vp, _vp, ctypes.c_int, _vp]
     L.mlb_synth_process_host.argtypes = [_vp, _vp, _vp, _vp, _vp, ctypes.c_int]
+    L.mlb_buses_create.argtypes = [ctypes.c_int, ctypes.c_int, _vp, _vp, _vp]
+    L.mlb_buses_destroy.argtypes = [_vp]
+    L.mlb_buses_sum_device.argtypes = [_vp, _vp, _vp, ctypes.c_int, ctypes.c_int, _vp]
+    L.mlb_synth_process_buses_host.argtypes = [_vp, _vp, _vp, _vp, _vp, ctypes.c_int]
     L.mlb_graph_process_host.argtypes = [_vp, _vp, _vp, _vp, ctypes.c_int]
     L.mlb_graph_last_kernel_ms.argtypes = [_vp, _vp]
     L.mlb_graph_last_host_slices.argtypes = [_vp]
@@ -377,6 +381,26 @@ class VoiceGraph:
                                             _ptr(mix) if want_mix else None, T))
         return out, mix
 
+    def process_events_buses_host(self, bank: "VoiceBank", buses: "Buses", events: np.ndarray,
+                                  out: Optional[np.ndarray] = None) -> np.ndarray:
+        """Contract E with per-instrument output (mlb_synth_process_buses_host): event records [T][V] in, the bus rows
+        [T][n_out][G][64] out -- each bus the strict-order sum of its voices' output rows (Synth::processVector).
+        The voice rows never leave the device."""
+        s, V = self.spec, self.n_voices
+        if not (isinstance(events, np.ndarray) and events.ndim == 2 and events.shape[1] == V and
+                events.dtype.itemsize == 72 and events.flags["C_CONTIGUOUS"]):
+            raise ValueError("process_events_buses_host: `events` must be a C-contiguous [T][V] array of 72-byte "
+                             "records")
+        T = int(events.shape[0])
+        shape = (T, s.n_out, buses.n_buses, BLOCK)
+        if out is None:
+            out = np.empty(shape, np.float32)
+        if not (isinstance(out, np.ndarray) and out.dtype == np.float32 and out.flags["C_CONTIGUOUS"] and
+                out.shape == shape):
+            raise ValueError(f"process_events_buses_host: `out` must be a C-contiguous float32 array of shape {shape}")
+        _check(lib().mlb_synth_process_buses_host(bank._h, self._h, buses._h, events.ctypes.data, _ptr(out), T))
+        return out
+
     def process_device(self, inp, out, mix, n_blocks: int, stream: int = 0) -> None:
         """Device pointers (torch tensors / ints); asynchronous on ``stream`` (cudaStream_t)."""
         _check(lib().mlb_graph_process_device(self._h, _ptr(inp), _ptr(out), _ptr(mix), int(n_blocks),
@@ -492,6 +516,39 @@ class VoiceBank:
     def process_device(self, events, out, n_blocks: int, row_mask: int = 0xFF, stream: int = 0) -> None:
         _check(lib().mlb_voices_process_device(self._h, _ptr(events), _ptr(out), int(n_blocks), row_mask,
                                                stream or None))
+
+
+class Buses:
+    """G per-instrument output buses over a V-voice bank (mlb_buses_*): bus g is the strict left-to-right sum, from
+    +0, of the voice rows [first[g], first[g] + count[g]) -- Synth::processVector (MLSynth.h:36-60) per instrument.
+    Ranges may be empty, leave gaps (MPE main voices) and overlap."""
+
+    def __init__(self, n_voices: int, first, count):
+        fv = np.ascontiguousarray(first, np.int32)
+        vc = np.ascontiguousarray(count, np.int32)
+        if fv.ndim != 1 or fv.shape != vc.shape:
+            raise ValueError(f"Buses: `first` and `count` must be 1-D of one length, got {fv.shape} and {vc.shape}")
+        self.n_voices, self.n_buses = int(n_voices), int(fv.shape[0])
+        h = ctypes.c_void_p()
+        _check(lib().mlb_buses_create(self.n_voices, self.n_buses, fv.ctypes.data, vc.ctypes.data, ctypes.byref(h)))
+        self._h = h
+
+    def close(self) -> None:
+        if self._h:
+            lib().mlb_buses_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def sum_device(self, rows, out, n_planes: int, n_blocks: int, stream: int = 0) -> None:
+        """Device buffers (torch tensors / ints): rows [T][P][V][64] -> out [T][P][G][64]; asynchronous on ``stream``,
+        one kernel launch, no allocation or synchronisation (capturable into a CUDA graph)."""
+        _check(lib().mlb_buses_sum_device(self._h, _ptr(rows), _ptr(out), int(n_planes), int(n_blocks),
+                                          stream or None))
 
 
 class ResamplerBank:

@@ -1,0 +1,64 @@
+// bus_kernel.cuh -- K10: per-instrument output buses, the voice sum of the reference's Synth::processVector
+// (source/app/MLSynth.h:36-60) for G instruments at once.
+//
+// A bus g is the voice range [first[g], first[g] + count[g]) of a V-voice bank.  For every block t, plane p and
+// sample n:  bus[t][p][g][n] = ((+0 + x[first]) + x[first + 1]) + ... + x[first + count - 1],  one binary32 add
+// per voice, round to nearest, subnormals kept -- what `outputs[i] = DSPVector{0.f}; ... outputs[i] += row`
+// does with the default isVoiceActive.  No tree, no atomics, no FTZ: the order is the contract.
+//
+// One warp per (t, p, g); lane l owns columns 2l and 2l + 1, so each voice row is one coalesced 256-byte warp
+// load and the bus row leaves as one 256-byte store.  The adds are serial per column; the loads are not:
+// kBusAhead rows are loaded (read-once, so not allocated in L1) before they are added in order.
+#pragma once
+#include "ops.cuh"
+
+namespace mlb
+{
+constexpr int kBusWarps = 8;  // (t, p, g) items per 256-thread CTA
+constexpr int kBusAhead = 8;  // voice rows in flight per warp
+
+struct BusArgs
+{
+  const float* rows;     // [T][P][V][64]
+  float* bus;            // [T][P][G][64]
+  const int32_t* first;  // [G]
+  const int32_t* count;  // [G]
+  int V, G;
+  long long n_items;     // T * P * G
+};
+
+MLB_DEV float2 ld_stream_f2(const float2* p)
+{
+  float2 r;
+  asm volatile("ld.global.nc.L1::no_allocate.v2.f32 {%0, %1}, [%2];" : "=f"(r.x), "=f"(r.y) : "l"(p));
+  return r;
+}
+
+__global__ void __launch_bounds__(32 * kBusWarps) bus_sum_kernel(BusArgs a)
+{
+  const long long w = (long long)blockIdx.x * kBusWarps + (threadIdx.x >> 5);
+  if (w >= a.n_items) return;
+  const int lane = threadIdx.x & 31;
+  const int g = (int)(w % a.G);
+  const long long tp = w / a.G;  // t * P + p
+  const int first = __ldg(a.first + g), count = __ldg(a.count + g);
+  const float2* src = reinterpret_cast<const float2*>(a.rows + ((size_t)tp * a.V + first) * MLB_BLOCK) + lane;
+  float2 acc = make_float2(0.f, 0.f);
+  for (int i = 0; i < count; i += kBusAhead)
+  {
+    float2 x[kBusAhead];
+#pragma unroll
+    for (int u = 0; u < kBusAhead; ++u)
+      if (i + u < count) x[u] = ld_stream_f2(src + (size_t)(i + u) * (MLB_BLOCK / 2));
+#pragma unroll
+    for (int u = 0; u < kBusAhead; ++u)
+      if (i + u < count)
+      {
+        acc.x = __fadd_rn(acc.x, x[u].x);
+        acc.y = __fadd_rn(acc.y, x[u].y);
+      }
+  }
+  reinterpret_cast<float2*>(a.bus + (size_t)w * MLB_BLOCK)[lane] = acc;
+}
+
+}  // namespace mlb

@@ -25,6 +25,7 @@
 #include "voice_kernel.cuh"
 #include "resample_kernel.cuh"
 #include "fdtd_kernel.cuh"
+#include "bus_kernel.cuh"
 #include "generic_kernel.cuh"
 
 using namespace mlb;
@@ -420,7 +421,7 @@ extern "C" void mlb_coeffs_fdn8(const float times[8], const float cutoffs[8], co
 // device
 
 static int g_device = -1;
-static std::atomic<int> g_live_handles{0};  // graphs + voice banks + resamplers + FDTD banks alive (they hold pointers of g_device)
+static std::atomic<int> g_live_handles{0};  // graphs + voice banks + resamplers + FDTD banks + bus layouts alive (they hold pointers of g_device)
 static int g_sm_count = 0;
 static size_t g_smem_optin = 0;
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
@@ -2483,40 +2484,54 @@ extern "C" int mlb_voices_process_host(mlb_voices* vb, const mlb_voice_events* e
 // Pipelined over TIME chunks -- blocks are contiguous in every buffer involved, and both the bank and
 // the graph carry their state from launch to launch -- so that the H2D copy of chunk c+1's records, the
 // two kernels of chunk c and the D2H copy of chunk c-1's output rows overlap.
-extern "C" int mlb_synth_process_host(mlb_voices* vb, mlb_graph* g, const mlb_voice_events* events_host,
-                                      float* out_host, float* mix_host, int n_blocks)
+// mlb_synth_process_buses_host runs the same pipeline with the bus kernel (K10) after the graph.
+
+// The checks both contract-E entry points share; *row_mask = the Voice rows the graph reads.
+static int synth_check(const mlb_voices* vb, const mlb_graph* g, const mlb_voice_events* events_host, int n_blocks,
+                       unsigned* row_mask)
 {
   if (!vb || !g || !events_host) return fail(MLB_ERR_INVALID, "null argument");
   if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive");
   if (vb->V != g->V) return fail(MLB_ERR_INVALID, "voice bank has %d voices, graph has %d", vb->V, g->V);
-  unsigned row_mask = 0;
+  *row_mask = 0;
   for (const mlb_node& n : g->nodes)
     if (n.op == MLB_OP_INPUT)
     {
       if (n.iarg < 0 || n.iarg >= MLB_VOICE_ROWS)
         return fail(MLB_ERR_INVALID, "graph INPUT plane %d is not a Voice row (0..%d)", n.iarg, MLB_VOICE_ROWS - 1);
-      row_mask |= 1u << n.iarg;
+      *row_mask |= 1u << n.iarg;
     }
-  if (!row_mask) return fail(MLB_ERR_INVALID, "graph reads no Voice row (no INPUT node)");
-  if (g->outs.empty() && (out_host || mix_host)) return fail(MLB_ERR_INVALID, "graph has no outputs");
-  int rc = ensure_init();
-  if (rc != MLB_OK) return rc;
-  const size_t V = (size_t)g->V, T = (size_t)n_blocks, n_out = g->outs.size();
-  const size_t plane = V * MLB_BLOCK * 4;
-  // rows of one chunk stay under ~1 GB (8 planes per block are addressed, only the masked ones are touched)
+  if (!*row_mask) return fail(MLB_ERR_INVALID, "graph reads no Voice row (no INPUT node)");
+  return MLB_OK;
+}
+
+// Blocks per time chunk: rows of one chunk stay under ~1 GB (8 planes per block are addressed, only the masked
+// ones are touched), and a call has at most kMaxHostSlices chunks.
+static int synth_chunk_blocks(const mlb_graph* g, int n_blocks)
+{
   int Tc = env_int("MLB_SYNTH_CHUNK_BLOCKS", 0);
-  if (Tc <= 0) Tc = (int)std::max<size_t>(1, ((size_t)1 << 30) / (MLB_VOICE_ROWS * plane));
+  if (Tc <= 0) Tc = (int)std::max<size_t>(1, ((size_t)1 << 30) / (MLB_VOICE_ROWS * (size_t)g->V * MLB_BLOCK * 4));
   Tc = std::min<int>(Tc, n_blocks);
-  Tc = std::max<int>(Tc, (n_blocks + mlb_graph::kMaxHostSlices - 1) / mlb_graph::kMaxHostSlices);
-  const size_t ev_bytes = T * V * sizeof(mlb_voice_events);
-  if ((rc = ensure_buf(reinterpret_cast<float**>(&vb->d_ev), &vb->ev_cap, ev_bytes)) != MLB_OK) return rc;
-  if ((rc = ensure_buf(&vb->d_out, &vb->out_cap, (size_t)Tc * MLB_VOICE_ROWS * plane)) != MLB_OK) return rc;
-  if (out_host && (rc = ensure_buf(&g->d_out, &g->out_cap, T * n_out * plane)) != MLB_OK) return rc;
-  if (mix_host && (rc = ensure_buf(&g->d_mix, &g->mix_cap, T * n_out * MLB_BLOCK * 4)) != MLB_OK) return rc;
+  return std::max<int>(Tc, (n_blocks + mlb_graph::kMaxHostSlices - 1) / mlb_graph::kMaxHostSlices);
+}
+
+// The time-chunk loop.  Per chunk [t0, t0 + tc) of Tc blocks: the records go up on g->s_h2d; on the graph's stream
+// the bank writes the rows the graph reads into vb->d_out, and run_chunk(t0, tc, s) launches what reads them; then,
+// if down_host, the chunk's tc * down_per_block floats of down_dev go down on g->s_d2h.  The caller drains the
+// streams (synth_drain) whatever this returns.
+template <class RunChunk>
+static int synth_pipeline(mlb_voices* vb, mlb_graph* g, const mlb_voice_events* events_host, int n_blocks,
+                          unsigned row_mask, int Tc, const float* down_dev, float* down_host, size_t down_per_block,
+                          RunChunk run_chunk)
+{
+  const size_t V = (size_t)g->V, T = (size_t)n_blocks;
+  int rc;
+  if ((rc = ensure_buf(reinterpret_cast<float**>(&vb->d_ev), &vb->ev_cap, T * V * sizeof(mlb_voice_events))) != MLB_OK)
+    return rc;
+  if ((rc = ensure_buf(&vb->d_out, &vb->out_cap, (size_t)Tc * MLB_VOICE_ROWS * V * MLB_BLOCK * 4)) != MLB_OK) return rc;
   const int saved_inputs = g->layout.n_inputs;
   g->layout.n_inputs = MLB_VOICE_ROWS;
   cudaStream_t s = g->stream;
-  rc = MLB_OK;
   int p = 0;
   for (size_t t0 = 0; t0 < T && rc == MLB_OK; t0 += (size_t)Tc, ++p)
   {
@@ -2532,33 +2547,159 @@ extern "C" int mlb_synth_process_host(mlb_voices* vb, mlb_graph* g, const mlb_vo
     }
     rc = mlb_voices_process_device(vb, vb->d_ev + t0 * V, vb->d_out, tc, row_mask, s);
     if (rc != MLB_OK) break;
-    rc = mlb_graph_process_device(g, vb->d_out, out_host ? g->d_out + t0 * n_out * V * MLB_BLOCK : nullptr,
-                                  mix_host ? g->d_mix + t0 * n_out * MLB_BLOCK : nullptr, tc, s);
+    rc = run_chunk(t0, tc, s);
     if (rc != MLB_OK) break;
-    if (out_host)
+    if (down_host)
     {
       ce = cudaEventRecord(g->ev_k[p], s);
       if (ce == cudaSuccess) ce = cudaStreamWaitEvent(g->s_d2h, g->ev_k[p], 0);
       if (ce == cudaSuccess)
-        ce = cudaMemcpyAsync(out_host + t0 * n_out * V * MLB_BLOCK, g->d_out + t0 * n_out * V * MLB_BLOCK,
-                             (size_t)tc * n_out * plane, cudaMemcpyDeviceToHost, g->s_d2h);
+        ce = cudaMemcpyAsync(down_host + t0 * down_per_block, down_dev + t0 * down_per_block,
+                             (size_t)tc * down_per_block * 4, cudaMemcpyDeviceToHost, g->s_d2h);
       if (ce != cudaSuccess) rc = fail(MLB_ERR_CUDA, "rows D2H: %s", cudaGetErrorString(ce));
     }
   }
   g->layout.n_inputs = saved_inputs;
   g->last_host_slices = p;
-  if (rc == MLB_OK && mix_host)
-  {
-    rc = mlb_graph_mix_wait(g, s);
-    if (rc == MLB_OK && cudaMemcpyAsync(mix_host, g->d_mix, T * n_out * MLB_BLOCK * 4, cudaMemcpyDeviceToHost, s) != cudaSuccess)
-      rc = fail(MLB_ERR_CUDA, "mix D2H failed");
-  }
-  // drain all three streams whatever happened: nothing may still touch the caller's buffers on return
+  return rc;
+}
+
+// Drain all three streams whatever happened: nothing may still touch the caller's buffers on return.
+static int synth_drain(mlb_graph* g, int rc)
+{
   cudaStreamSynchronize(g->s_h2d);
-  cudaError_t e1 = cudaStreamSynchronize(s), e2 = cudaStreamSynchronize(g->s_d2h);
+  cudaError_t e1 = cudaStreamSynchronize(g->stream), e2 = cudaStreamSynchronize(g->s_d2h);
   if (rc == MLB_OK && (e1 != cudaSuccess || e2 != cudaSuccess))
     rc = fail(MLB_ERR_CUDA, "synth pipeline: %s", cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
   return rc;
+}
+
+extern "C" int mlb_synth_process_host(mlb_voices* vb, mlb_graph* g, const mlb_voice_events* events_host,
+                                      float* out_host, float* mix_host, int n_blocks)
+{
+  unsigned row_mask;
+  int rc = synth_check(vb, g, events_host, n_blocks, &row_mask);
+  if (rc != MLB_OK) return rc;
+  if (g->outs.empty() && (out_host || mix_host)) return fail(MLB_ERR_INVALID, "graph has no outputs");
+  if ((rc = ensure_init()) != MLB_OK) return rc;
+  const size_t V = (size_t)g->V, T = (size_t)n_blocks, n_out = g->outs.size();
+  const int Tc = synth_chunk_blocks(g, n_blocks);
+  if (out_host && (rc = ensure_buf(&g->d_out, &g->out_cap, T * n_out * V * MLB_BLOCK * 4)) != MLB_OK) return rc;
+  if (mix_host && (rc = ensure_buf(&g->d_mix, &g->mix_cap, T * n_out * MLB_BLOCK * 4)) != MLB_OK) return rc;
+  rc = synth_pipeline(vb, g, events_host, n_blocks, row_mask, Tc, g->d_out, out_host, n_out * V * MLB_BLOCK,
+                      [&](size_t t0, int tc, cudaStream_t s)
+                      {
+                        return mlb_graph_process_device(g, vb->d_out,
+                                                        out_host ? g->d_out + t0 * n_out * V * MLB_BLOCK : nullptr,
+                                                        mix_host ? g->d_mix + t0 * n_out * MLB_BLOCK : nullptr, tc, s);
+                      });
+  if (rc == MLB_OK && mix_host)
+  {
+    rc = mlb_graph_mix_wait(g, g->stream);
+    if (rc == MLB_OK &&
+        cudaMemcpyAsync(mix_host, g->d_mix, T * n_out * MLB_BLOCK * 4, cudaMemcpyDeviceToHost, g->stream) != cudaSuccess)
+      rc = fail(MLB_ERR_CUDA, "mix D2H failed");
+  }
+  return synth_drain(g, rc);
+}
+
+// ------------------------------------------------------------------------------------------
+// Per-instrument output buses (K10, bus_kernel.cuh)
+
+struct mlb_buses
+{
+  int V = 0, G = 0;
+  int32_t* d_table = nullptr;  // [2][G]: first voice, voice count
+  float* d_out = nullptr;      // bus rows of mlb_synth_process_buses_host, [T][n_out][G][64]
+  size_t out_cap = 0;
+};
+
+extern "C" int mlb_buses_destroy(mlb_buses* b)
+{
+  if (!b) return MLB_OK;
+  cudaFree(b->d_table);
+  cudaFree(b->d_out);
+  delete b;
+  --g_live_handles;
+  return MLB_OK;
+}
+
+extern "C" int mlb_buses_create(int n_voices, int n_buses, const int32_t* first_voice, const int32_t* voice_count,
+                                mlb_buses** out)
+{
+  if (!out) return fail(MLB_ERR_INVALID, "out is null");
+  *out = nullptr;
+  if (n_voices <= 0) return fail(MLB_ERR_INVALID, "n_voices must be positive (got %d)", n_voices);
+  if (n_buses < 1) return fail(MLB_ERR_INVALID, "n_buses must be positive (got %d)", n_buses);
+  if (!first_voice || !voice_count) return fail(MLB_ERR_INVALID, "null layout table");
+  for (int g = 0; g < n_buses; ++g)
+    if (first_voice[g] < 0 || voice_count[g] < 0 || (int64_t)first_voice[g] + voice_count[g] > n_voices)
+      return fail(MLB_ERR_INVALID, "bus %d: first voice %d, count %d is not a range of the %d voices", g,
+                  first_voice[g], voice_count[g], n_voices);
+  int rc = ensure_init();
+  if (rc != MLB_OK) return rc;
+  mlb_buses* b = new mlb_buses;
+  ++g_live_handles;
+  b->V = n_voices, b->G = n_buses;
+  const size_t bytes = (size_t)n_buses * sizeof(int32_t);
+  if (cudaMalloc(&b->d_table, 2 * bytes) != cudaSuccess)
+  {
+    mlb_buses_destroy(b);
+    return fail(MLB_ERR_ALLOC, "cudaMalloc of bus layout failed");
+  }
+  if (cudaMemcpy(b->d_table, first_voice, bytes, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy(b->d_table + n_buses, voice_count, bytes, cudaMemcpyHostToDevice) != cudaSuccess)
+  {
+    mlb_buses_destroy(b);
+    return fail(MLB_ERR_CUDA, "upload of bus layout failed");
+  }
+  *out = b;
+  return MLB_OK;
+}
+
+extern "C" int mlb_buses_sum_device(mlb_buses* b, const float* rows_dev, float* bus_dev, int n_planes, int n_blocks,
+                                    void* stream)
+{
+  if (!b || !rows_dev || !bus_dev) return fail(MLB_ERR_INVALID, "null argument");
+  if (n_planes <= 0) return fail(MLB_ERR_INVALID, "n_planes must be positive (got %d)", n_planes);
+  if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive (got %d)", n_blocks);
+  BusArgs a;
+  a.rows = rows_dev, a.bus = bus_dev, a.first = b->d_table, a.count = b->d_table + b->G;
+  a.V = b->V, a.G = b->G;
+  a.n_items = (long long)n_blocks * n_planes * b->G;
+  const long long grid = (a.n_items + kBusWarps - 1) / kBusWarps;
+  if (grid > 0x7FFFFFFFLL) return fail(MLB_ERR_INVALID, "%lld bus rows exceed one launch", a.n_items);
+  bus_sum_kernel<<<(unsigned)grid, 32 * kBusWarps, 0, (cudaStream_t)stream>>>(a);
+  ++g_launches;
+  CU_CHECK(cudaGetLastError());
+  return MLB_OK;
+}
+
+// Contract E with per-instrument output: the graph's rows of a chunk go to a device scratch of one chunk (g->d_out),
+// the bus kernel sums them on the same stream right after the graph, and only the bus rows come back.
+extern "C" int mlb_synth_process_buses_host(mlb_voices* vb, mlb_graph* g, mlb_buses* b,
+                                            const mlb_voice_events* events_host, float* bus_host, int n_blocks)
+{
+  unsigned row_mask;
+  int rc = synth_check(vb, g, events_host, n_blocks, &row_mask);
+  if (rc != MLB_OK) return rc;
+  if (!b || !bus_host) return fail(MLB_ERR_INVALID, "null argument");
+  if (b->V != g->V) return fail(MLB_ERR_INVALID, "buses are laid over %d voices, graph has %d", b->V, g->V);
+  if (g->outs.empty()) return fail(MLB_ERR_INVALID, "graph has no outputs");
+  if ((rc = ensure_init()) != MLB_OK) return rc;
+  const size_t V = (size_t)g->V, T = (size_t)n_blocks, n_out = g->outs.size(), G = (size_t)b->G;
+  const int Tc = synth_chunk_blocks(g, n_blocks);
+  if ((rc = ensure_buf(&g->d_out, &g->out_cap, (size_t)Tc * n_out * V * MLB_BLOCK * 4)) != MLB_OK) return rc;
+  if ((rc = ensure_buf(&b->d_out, &b->out_cap, T * n_out * G * MLB_BLOCK * 4)) != MLB_OK) return rc;
+  rc = synth_pipeline(vb, g, events_host, n_blocks, row_mask, Tc, b->d_out, bus_host, n_out * G * MLB_BLOCK,
+                      [&](size_t t0, int tc, cudaStream_t s)
+                      {
+                        int r = mlb_graph_process_device(g, vb->d_out, g->d_out, nullptr, tc, s);
+                        if (r != MLB_OK) return r;
+                        return mlb_buses_sum_device(b, g->d_out, b->d_out + t0 * n_out * G * MLB_BLOCK, (int)n_out, tc,
+                                                    s);
+                      });
+  return synth_drain(g, rc);
 }
 
 // ------------------------------------------------------------------------------------------

@@ -685,6 +685,17 @@ def synth_events(n_voices: int, n_blocks: int, seed: int = 2, density: float = 0
     return np.ascontiguousarray(np.tile(base, (1, reps))[:, :n_voices])
 
 
+def instrument_buses(n_instruments: int, polyphony: int, mpe: bool = False):
+    """The bus layout (first voice, voice count; int32 [G] each) of a bank of n_instruments Synths with `polyphony`
+    voices each, for api.Buses.  MIDI: instrument k is voices [k poly, (k + 1) poly).  MPE: instrument k owns
+    poly + 1 voices, of which the first, k (poly + 1), is its main voice; Synth sums getInputVoice(v) = voices[v + 1]
+    (MLEventsToSignals.h:184), so the bus skips it: [k (poly + 1) + 1, (k + 1) (poly + 1))."""
+    k = np.arange(n_instruments, dtype=np.int64)
+    stride = polyphony + 1 if mpe else polyphony
+    first = (k * stride + (1 if mpe else 0)).astype(np.int32)
+    return first, np.full(n_instruments, polyphony, np.int32)
+
+
 # ---- random voice graphs (tests): any DAG of the op table, for checker-vs-checker and GPU-vs-checker runs ----
 
 def random_graph_workload(seed: int, n_voices: int = 37, n_nodes: int = 24, hw_approx: bool = True,

@@ -2,13 +2,14 @@
 """Kernel-resident timing of everything except the headline: BASELINE.json configurations 2-5, the
 SURVEY 8(f) workloads (config 6 = Aaltoverb x V, the EventsToSignals::Voice bank) and the elementwise maps.
 
-    python tools/bench_configs.py [--steps K] [--only 2,3,4,5,6,voices,map,fdtd] [--generic] [--cpu]
+    python tools/bench_configs.py [--steps K] [--only 2,3,4,5,6,voices,map,fdtd,buses] [--generic] [--cpu]
 
 Prints one JSON line per configuration: kernel name, mean CUDA-event kernel time, algorithmic
 bytes per launch (SURVEY.md 8d / DESIGN.md), achieved GB/s and fraction of the measured HBM peak.
 --cpu also times the reference (oracle/_ref) on the box's host cores for config 6, the Voice bank and the FDTD
 membranes.  The FDTD lines (K9) are compute-bound: they report instance-samples/s and the share of the FP32 issue
-ceiling instead of bytes.
+ceiling instead of bytes.  The bus lines (K10) report bytes against the data-sheet HBM bandwidth, and contract E
+with bus output against the rows-out and mix-only paths in voice-samples/s.
 Not the headline benchmark (that is bench.py / config A).
 """
 import argparse
@@ -28,7 +29,7 @@ def main():
     from madronalib_b200 import api, workloads as wl
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
-    ap.add_argument("--only", default="2,3,swept,4,5,6,voices,map,fdtd")
+    ap.add_argument("--only", default="2,3,swept,4,5,6,voices,map,fdtd,buses")
     ap.add_argument("--generic", action="store_true", help="force the graph interpreter kernel")
     ap.add_argument("--cpu", action="store_true",
                     help="also time the reference (oracle/_ref, all host threads) on config 6, the Voice bank "
@@ -117,6 +118,8 @@ def main():
         del d_ev, d_rows
     if "fdtd" in only:
         bench_fdtd(api, wl, torch, dev, args.steps, args.cpu)
+    if "buses" in only:
+        bench_buses(api, wl, torch, dev, args.steps)
     if args.cpu:
         # the reference itself on this box's host cores (oracle/_ref; checker code, used here only as a baseline)
         import time
@@ -266,6 +269,116 @@ def bench_fdtd(api, wl, torch, dev, steps, cpu):
                               "note": "the example's own processFDTDModel under UsingFlushDenormalsToZero "
                                       "(oracle/_ref/libmlfdtd.so), same inputs"}), flush=True)
         del d_in, d_out
+
+
+HBM_DATASHEET_GBS = 3350.0  # H100 SXM data sheet (700 W card), not a measured peak
+
+
+def bench_buses(api, wl, torch, dev, steps):
+    """K10 alone, rows resident on the device: mean of `steps` CUDA-event-timed launches after 3 warm-up launches;
+    algorithmic bytes = every voice row of every bus read once + the bus rows written.  Parity of up to 64 sampled
+    buses (all blocks; for G = 1, the first and last block) against the plain-C port.  Then contract E at
+    65 536 voices x 64 vectors as 4 096 instruments x 16 voices: rows out, mix bus only, and bus rows out."""
+    from oracle import bus_bindings as bb
+    T = 64
+    facts = gpu_facts()
+    shapes = [(4096, 16, 1), (4096, 16, 2), (16384, 4, 1), (16384, 4, 2), (1, 65536, 1)]
+    for G, poly, P in shapes:
+        V = G * poly
+        first, count = wl.instrument_buses(G, poly)
+        rows = torch.randn((T, P, V, 64), dtype=torch.float32, device=dev)
+        bus = torch.empty((T, P, G, 64), dtype=torch.float32, device=dev)
+        b = api.Buses(V, first, count)
+        sh = torch.cuda.current_stream().cuda_stream
+        for _ in range(3):
+            b.sum_device(rows, bus, P, T, sh)
+        times = []
+        for _ in range(steps):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            b.sum_device(rows, bus, P, T, sh)
+            e1.record()
+            torch.cuda.synchronize()
+            times.append(e0.elapsed_time(e1))
+        b.close()
+        sel = np.unique(np.linspace(0, G - 1, min(G, 64)).astype(np.int64))
+        sel_t = np.arange(T) if G > 1 else np.array([0, T - 1])
+        voices = (first[sel, None] + np.arange(poly)[None, :]).reshape(-1)
+        sub = rows[torch.from_numpy(sel_t).to(dev)][:, :, torch.from_numpy(voices).to(dev)].cpu().numpy()
+        want = bb.port_buses(sub, *wl.instrument_buses(len(sel), poly))
+        got = bus[torch.from_numpy(sel_t).to(dev)][:, :, torch.from_numpy(sel).to(dev)].cpu().numpy()
+        mism = int(((got.view(np.uint32) != want.view(np.uint32)) & ~(np.isnan(got) & np.isnan(want))).sum())
+        ms = float(np.mean(times))
+        nbytes = 4.0 * 64 * T * P * (V + G)
+        print(json.dumps({
+            "config": "buses_%dx%d_p%d" % (G, poly, P), "kernel": "bus_sum_kernel", "buses": G, "voices_per_bus": poly,
+            "planes": P, "blocks": T, "kernel_ms": ms, "algorithmic_bytes": nbytes,
+            "achieved_gbs": nbytes / (ms * 1e-3) / 1e9,
+            "frac_of_datasheet_hbm": nbytes / (ms * 1e-3) / 1e9 / HBM_DATASHEET_GBS,
+            "datasheet_note": "3.35 TB/s, H100 SXM data sheet", **facts,
+            "parity_buses": int(len(sel)), "parity_blocks": int(len(sel_t)), "parity_checker": "plain-C port",
+            "mismatches": mism}), flush=True)
+        del rows, bus
+        torch.cuda.empty_cache()
+    bench_contract_e_buses(api, wl, torch, facts)
+
+
+def bench_contract_e_buses(api, wl, torch, facts, n_calls=5):
+    """Contract E, 65 536 voices x 64 vectors of config A, pinned host buffers, host clock around calls that return
+    finished: rows + mix out, mix only, bus rows of 4 096 x 16 instruments out.  Parity of 16 buses of the last
+    call against port(bank) -> port(graph) -> port(buses), the events replayed for every call made."""
+    import time
+    from oracle import bindings, bus_bindings as bb
+    V, T, G, poly = 65536, 64, 4096, 16
+    w = wl.config_a(V)
+    prm = wl.synth_bank_params(V)
+    ev_np = wl.synth_events(V, T)
+    h_ev = torch.empty(ev_np.nbytes, dtype=torch.uint8).pin_memory()
+    h_ev.numpy()[:] = ev_np.view(np.uint8).reshape(-1)
+    ev = h_ev.numpy().view(ev_np.dtype).reshape(T, V)
+    h_out = torch.empty((T, 1, V, 64), dtype=torch.float32).pin_memory().numpy()
+    h_mix = torch.empty((T, 1, 64), dtype=torch.float32).pin_memory().numpy()
+    h_bus = torch.empty((T, 1, G, 64), dtype=torch.float32).pin_memory().numpy()
+    first, count = wl.instrument_buses(G, poly)
+    vb = api.VoiceBank(48000.0, *prm)
+    g = api.VoiceGraph(w.spec, V)
+    b = api.Buses(V, first, count)
+    g.set_coefs(w.coef)
+    g.set_state(w.state)
+    legs = (("contract_E_rows", lambda: g.process_events_host(vb, ev, want_out=True, want_mix=True, out=h_out, mix=h_mix),
+             h_out.nbytes + h_mix.nbytes),
+            ("contract_E_mix", lambda: g.process_events_host(vb, ev, want_out=False, want_mix=True, mix=h_mix),
+             h_mix.nbytes),
+            ("contract_E_buses", lambda: g.process_events_buses_host(vb, b, ev, out=h_bus), h_bus.nbytes))
+    calls = 0
+    for name, call, down in legs:
+        call()
+        t0 = time.perf_counter()
+        for _ in range(n_calls):
+            call()
+        dt = time.perf_counter() - t0
+        calls += 1 + n_calls
+        print(json.dumps({"config": name, "voices": V, "blocks": T, "ms_per_call": 1e3 * dt / n_calls,
+                          "voice_samples_per_s": V * T * 64 * n_calls / dt, "h2d_bytes_per_call": int(ev.nbytes),
+                          "d2h_bytes_per_call": int(down), "time_chunks": g.last_host_slices,
+                          "kernels": "voice_bank_kernel -> " + g.kernel_name +
+                                     (" -> bus_sum_kernel" if name.endswith("buses") else ""), **facts}), flush=True)
+    for h in (g, vb, b):
+        h.close()
+    sel = np.linspace(0, G - 1, 16).astype(np.int64)
+    voices = (first[sel, None] + np.arange(poly)[None, :]).reshape(-1)
+    rows, _ = bindings.port_voice_bank().run(48000.0, *(p_[voices] for p_ in prm),
+                                             np.ascontiguousarray(np.tile(ev[:, voices], (calls, 1))),
+                                             nthreads=os.cpu_count() or 1)
+    out, _, _ = bindings.PortOracle().run(w.spec, len(voices), T * calls, np.ascontiguousarray(rows[:, 0:1]),
+                                          np.ascontiguousarray(w.state[:, voices]),
+                                          np.ascontiguousarray(w.coef[:, voices]), nthreads=os.cpu_count() or 1)
+    want = bb.port_buses(np.ascontiguousarray(out[T * (calls - 1):]), *wl.instrument_buses(len(sel), poly))
+    got = np.ascontiguousarray(h_bus[:, :, sel])
+    mism = int(((got.view(np.uint32) != want.view(np.uint32)) & ~(np.isnan(got) & np.isnan(want))).sum())
+    print(json.dumps({"config": "contract_E_buses_parity", "buses": int(len(sel)), "blocks": T,
+                      "calls_replayed": calls, "checker": "port bank -> port graph -> port buses",
+                      "mismatches": mism}), flush=True)
 
 
 if __name__ == "__main__":
