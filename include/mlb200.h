@@ -349,13 +349,14 @@ void mlb_interpolate_coeffs_linear(const float* c0, const float* c1, int n_coeff
 
 /* ---- device / context ---- */
 /* One device per process (the multi-GPU model is one process per GPU): mlb_init(other) while graphs, voice
- * banks, resamplers, FDTD banks or bus layouts of the current device are alive returns MLB_ERR_INVALID.  Entry points make the
- * library's device current on the calling thread. */
+ * banks, bus layouts, resamplers, FDTD banks or mix buses of the current device are alive returns MLB_ERR_INVALID.
+ * Entry points make the library's device current on the calling thread. */
 int mlb_init(int device);          /* select device, check sm_90; MLB_ERR_NO_DEVICE if absent */
 int mlb_device_count(void);        /* 0 when no GPU: callers must fail loudly, not fall back */
 const char* mlb_last_error(void);  /* thread-local message of the last failing call */
 int mlb_abi_version(void);
 long long mlb_kernel_launches(void); /* count of kernels this library launched (process-wide) */
+int mlb_live_handles(void);          /* handles of the kinds mlb_init counts that are alive now (process-wide) */
 
 /* ---- block-rate resamplers (SURVEY 8f row 4) -------------------------------------------------
  * Upsampler(octaves) / Downsampler(octaves), source/DSP/MLDSPFilters.h:1316-1473: cascades of

@@ -179,6 +179,11 @@ def kernel_launches() -> int:
     return int(lib().mlb_kernel_launches())
 
 
+def live_handles() -> int:
+    """Graphs, voice banks, bus layouts, resamplers, FDTD banks and mix buses alive in this process."""
+    return int(lib().mlb_live_handles())
+
+
 # ---- coefficient design (host libm; same calls as the reference's makeCoeffs) ----
 _NCOEF = {"lopass": 3, "hipass": 4, "bandpass": 3, "loshelf": 5, "hishelf": 6, "bell": 4, "onepole": 2,
           "peak": 2, "rms": 2, "adsr": 4, "glide": 2, "sample_glide": 2}
@@ -282,8 +287,29 @@ def plan(spec: GraphSpec, n_voices: int, flags: int = 0):
     return list(stage)[:n], int(ns.value), int(rows.value)
 
 
-class VoiceGraph:
+class _Handle:
+    """Owner of one library handle ``_h``: ``close()`` (a no-op once closed) or the garbage collector hands it to the
+    library function named ``_destroy``."""
+
+    _h = None
+    _destroy = ""
+
+    def close(self) -> None:
+        if self._h:
+            getattr(lib(), self._destroy)(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class VoiceGraph(_Handle):
     """Device-resident bank of ``n_voices`` identical graphs (one voice per CUDA lane)."""
+
+    _destroy = "mlb_graph_destroy"
 
     def __init__(self, spec: GraphSpec, n_voices: int, flags: int = FLAG_EXACT):
         self.spec = spec
@@ -297,17 +323,6 @@ class VoiceGraph:
         _check(L.mlb_graph_layout_of(self._h, ctypes.byref(lay)))
         assert (lay.n_state_words, lay.n_coef_words, lay.n_inputs) == (spec.n_state, spec.n_coef,
                                                                        spec.n_in)
-
-    def close(self) -> None:
-        if self._h:
-            lib().mlb_graph_destroy(self._h)
-            self._h = _vp()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     @property
     def kernel_name(self) -> str:
@@ -468,9 +483,11 @@ class MixBus:
             self._h = _vp()
 
 
-class VoiceBank:
+class VoiceBank(_Handle):
     """V x EventsToSignals::Voice on the device (SURVEY 8f row 3): per-voice event records in,
     the 8 control rows (pitch, gate, voice, z, x, y, mod, elapsed time) out."""
+
+    _destroy = "mlb_voices_destroy"
 
     ROWS = 8
 
@@ -486,17 +503,6 @@ class VoiceBank:
         _check(lib().mlb_voices_create(self.n_voices, sample_rate, vi.ctypes.data, gs.ctypes.data, da.ctypes.data,
                                        pb.ctypes.data, flags, ctypes.byref(h)))
         self._h = h
-
-    def close(self) -> None:
-        if self._h:
-            lib().mlb_voices_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def set_main_voices(self, main_voice) -> None:
         """MPE: main_voice[v] = bank index of voice v's main voice, or -1."""
@@ -518,10 +524,12 @@ class VoiceBank:
                                                stream or None))
 
 
-class Buses:
+class Buses(_Handle):
     """G per-instrument output buses over a V-voice bank (mlb_buses_*): bus g is the strict left-to-right sum, from
     +0, of the voice rows [first[g], first[g] + count[g]) -- Synth::processVector (MLSynth.h:36-60) per instrument.
     Ranges may be empty, leave gaps (MPE main voices) and overlap."""
+
+    _destroy = "mlb_buses_destroy"
 
     def __init__(self, n_voices: int, first, count):
         fv = np.ascontiguousarray(first, np.int32)
@@ -533,17 +541,6 @@ class Buses:
         _check(lib().mlb_buses_create(self.n_voices, self.n_buses, fv.ctypes.data, vc.ctypes.data, ctypes.byref(h)))
         self._h = h
 
-    def close(self) -> None:
-        if self._h:
-            lib().mlb_buses_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
     def sum_device(self, rows, out, n_planes: int, n_blocks: int, stream: int = 0) -> None:
         """Device buffers (torch tensors / ints): rows [T][P][V][64] -> out [T][P][G][64]; asynchronous on ``stream``,
         one kernel launch, no allocation or synchronisation (capturable into a CUDA graph)."""
@@ -551,8 +548,10 @@ class Buses:
                                           stream or None))
 
 
-class ResamplerBank:
+class ResamplerBank(_Handle):
     """Upsampler(octaves) / Downsampler(octaves) x V (SURVEY 8f row 4).  direction: 0 up, 1 down."""
+
+    _destroy = "mlb_resampler_destroy"
 
     UP, DOWN = 0, 1
 
@@ -561,17 +560,6 @@ class ResamplerBank:
         h = ctypes.c_void_p()
         _check(lib().mlb_resampler_create(direction, octaves, n_voices, ctypes.byref(h)))
         self._h = h
-
-    def close(self) -> None:
-        if self._h:
-            lib().mlb_resampler_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def clear(self) -> None:
         _check(lib().mlb_resampler_clear(self._h))
@@ -588,9 +576,11 @@ class ResamplerBank:
         return out[:n.value]
 
 
-class FDTDBank:
+class FDTDBank(_Handle):
     """V x the reference's FDTD membrane (FDTDState + processFDTDModel, examples/audio-and-midi/fdtd.cpp): per
     block, an excitation row and a frequency row (cycles per sample) in, the two pickup rows L, R out."""
+
+    _destroy = "mlb_fdtd_destroy"
 
     FTZ = 1  # MLB_FDTD_FTZ: every FP op flushes subnormals, as under UsingFlushDenormalsToZero
     SIZE = 16
@@ -602,17 +592,6 @@ class FDTDBank:
         _check(lib().mlb_fdtd_create(self.n_instances, sample_rate, self.in_planes, excite_plane, freq_plane, flags,
                                      ctypes.byref(h)))
         self._h = h
-
-    def close(self) -> None:
-        if self._h:
-            lib().mlb_fdtd_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def clear(self) -> None:
         _check(lib().mlb_fdtd_clear(self._h))
@@ -649,8 +628,10 @@ class _Event(ctypes.Structure):
                 ("time", ctypes.c_int32), ("value1", ctypes.c_float), ("value2", ctypes.c_float)]
 
 
-class EventRouter:
+class EventRouter(_Handle):
     """EventsToSignals' event routing (host only, no GPU needed): events in, per-voice records out."""
+
+    _destroy = "mlb_router_destroy"
 
     MIDI, MPE = 0, 1
     NOTE_ON, NOTE_OFF, SUSTAIN_PEDAL, CONTROLLER, PITCH_BEND, NOTE_PRESSURE, CHANNEL_PRESSURE = 1, 4, 5, 6, 7, 8, 9
@@ -662,17 +643,6 @@ class EventRouter:
         if unison:
             lib().mlb_router_set_unison(self._h, 1)
         self.n_records = lib().mlb_router_record_count(self._h)
-
-    def close(self) -> None:
-        if self._h:
-            lib().mlb_router_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def add_event(self, type: int, channel: int, source_idx: int, time: int, value1: float = 0.0,
                   value2: float = 0.0) -> None:

@@ -15,8 +15,11 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <string>
+#include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "../../include/mlb200.h"
@@ -54,9 +57,112 @@ static int fail(int code, const char* fmt, ...)
                   __FILE__, __LINE__);                                                      \
   } while (0)
 
+// return the MLB_* code of a failing call of this library
+#define MLB_TRY(expr)                \
+  do                                 \
+  {                                  \
+    const int rc__ = (expr);         \
+    if (rc__ != MLB_OK) return rc__; \
+  } while (0)
+
+// ------------------------------------------------------------------------------------------
+// owners of device memory, streams, events and live-handle counts: move-only, failures reported by the explicit
+// alloc / create calls (no exception crosses the C ABI).  A default-constructed owner makes no CUDA runtime call,
+// not even when it is destroyed: mlb_graph_plan builds a host-only graph.
+
+// graphs, voice banks, bus layouts, resamplers, FDTD banks and mix buses alive (they hold pointers of g_device)
+static std::atomic<int> g_live_handles{0};
+
+// One cudaMalloc allocation of T and its size in bytes.
+template <class T>
+class DevBuf
+{
+ public:
+  DevBuf() = default;
+  DevBuf(DevBuf&& o) noexcept { *this = std::move(o); }
+  DevBuf& operator=(DevBuf&& o) noexcept { std::swap(p_, o.p_); std::swap(bytes_, o.bytes_); return *this; }
+  ~DevBuf() { reset(); }
+  // frees the old allocation first; empty after a failure
+  int alloc(size_t bytes, const char* what)
+  {
+    reset();
+    const cudaError_t e = cudaMalloc(&p_, bytes);
+    if (e != cudaSuccess)
+    {
+      p_ = nullptr;
+      cudaGetLastError();
+      return fail(MLB_ERR_ALLOC, "cudaMalloc of %zu B %s failed: %s", bytes, what, cudaGetErrorString(e));
+    }
+    bytes_ = bytes;
+    return MLB_OK;
+  }
+  // grow only: nothing is copied
+  int ensure(size_t bytes, const char* what) { return bytes <= bytes_ ? MLB_OK : alloc(bytes, what); }
+  void reset()
+  {
+    if (p_) cudaFree(p_);
+    p_ = nullptr, bytes_ = 0;
+  }
+  T* get() const { return p_; }
+  size_t bytes() const { return bytes_; }
+
+ private:
+  T* p_ = nullptr;
+  size_t bytes_ = 0;
+};
+
+// One cudaStream_t or cudaEvent_t.  create() is a no-op once it has succeeded, so that a handle can create what it
+// needs on first use (mlb_graph_set_mix_async).
+template <class H>
+class CudaObj
+{
+ public:
+  CudaObj() = default;
+  CudaObj(CudaObj&& o) noexcept { std::swap(h_, o.h_); }
+  CudaObj& operator=(CudaObj&& o) noexcept { std::swap(h_, o.h_); return *this; }
+  ~CudaObj() { if (h_) destroy(h_); }
+  int create(unsigned flags)
+  {
+    const cudaError_t e = h_ ? cudaSuccess : make(&h_, flags);
+    if (e == cudaSuccess) return MLB_OK;
+    h_ = nullptr;
+    const char* kind = std::is_same<H, cudaStream_t>::value ? "stream" : "event";
+    return fail(MLB_ERR_CUDA, "creating a CUDA %s failed: %s", kind, cudaGetErrorString(e));
+  }
+  H get() const { return h_; }
+
+ private:
+  static cudaError_t make(cudaStream_t* s, unsigned flags) { return cudaStreamCreateWithFlags(s, flags); }
+  static cudaError_t make(cudaEvent_t* e, unsigned flags) { return cudaEventCreateWithFlags(e, flags); }
+  static void destroy(cudaStream_t s) { cudaStreamDestroy(s); }
+  static void destroy(cudaEvent_t e) { cudaEventDestroy(e); }
+  H h_ = nullptr;
+};
+using Stream = CudaObj<cudaStream_t>;
+using Event = CudaObj<cudaEvent_t>;
+
+// A handle's place in g_live_handles, from arm() until destruction.  Only the *_create entry points arm it.
+class LiveCount
+{
+ public:
+  LiveCount() = default;
+  LiveCount(LiveCount&& o) noexcept { std::swap(armed_, o.armed_); }
+  LiveCount& operator=(LiveCount&& o) noexcept { std::swap(armed_, o.armed_); return *this; }
+  ~LiveCount() { if (armed_) --g_live_handles; }
+  void arm()
+  {
+    if (!armed_) ++g_live_handles;
+    armed_ = true;
+  }
+
+ private:
+  bool armed_ = false;
+};
+
 extern "C" const char* mlb_last_error(void) { return g_err; }
 extern "C" int mlb_abi_version(void) { return MLB_ABI_VERSION; }
 extern "C" long long mlb_kernel_launches(void) { return g_launches.load(); }
+extern "C" int mlb_live_handles(void) { return g_live_handles.load(); }
 
 // ------------------------------------------------------------------------------------------
 // op metadata and graph layout (host only)
@@ -421,7 +527,6 @@ extern "C" void mlb_coeffs_fdn8(const float times[8], const float cutoffs[8], co
 // device
 
 static int g_device = -1;
-static std::atomic<int> g_live_handles{0};  // graphs + voice banks + resamplers + FDTD banks + bus layouts alive (they hold pointers of g_device)
 static int g_sm_count = 0;
 static size_t g_smem_optin = 0;
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
@@ -648,6 +753,17 @@ enum GraphKind
 
 struct mlb_graph
 {
+  // declared first, so released last: the buffers below are freed first, and cudaFree waits for the device
+  LiveCount live;
+  static constexpr int kMaxHostSlices = 64;
+  Stream stream, s_h2d, s_d2h;  // staging for the host entry point
+  Event ev_up[kMaxHostSlices], ev_k[kMaxHostSlices];
+  Event ev0, ev1;
+  // asynchronous mix bus (mlb_graph_set_mix_async): mix_reduce_kernel (and the multi-GPU exchange) run on s_mix,
+  // beside the next call's chain kernel; the per-group partials are double-buffered by call parity
+  Stream s_mix;
+  Event ev_main, ev_mixdone[4];
+
   std::vector<mlb_node> nodes;
   std::vector<int32_t> outs;
   std::vector<int32_t> st_off, co_off;
@@ -659,8 +775,8 @@ struct mlb_graph
   std::string kernel_name;
 
   // device SoA
-  uint32_t* d_state = nullptr;
-  float* d_coef = nullptr;
+  DevBuf<uint32_t> d_state;
+  DevBuf<float> d_coef;
   std::vector<float> h_coef;  // host mirror (ring sizing, FDN descriptors)
 
   // fused chain
@@ -672,54 +788,41 @@ struct mlb_graph
 
   // generic interpreter
   std::vector<GNode> gnodes;   // stage programs back to back (imports + nodes)
-  GNode* d_gnodes = nullptr;
+  DevBuf<GNode> d_gnodes;
   int scratch_slot = 0;
   std::vector<GStage> gstages;
-  GStage* d_gstages = nullptr;
+  DevBuf<GStage> d_gstages;
   int n_stages = 1, n_chan = 0;
-  unsigned* d_gsync = nullptr;  // [0] ticket, [1 + s*G + g] blocks finished by stage s of group g
-  float* d_chan = nullptr;      // channel planes [T][n_chan][V][64]
-  size_t chan_cap = 0;
+  DevBuf<unsigned> d_gsync;  // [0] ticket, [1 + s*G + g] blocks finished by stage s of group g
+  DevBuf<float> d_chan;      // channel planes [T][n_chan][V][64]
 
   int n_slots = 0;
 
   // FDN delay memory
   int fdn_node = -1;
-  float* d_ring = nullptr;
-  float* d_carry = nullptr;
+  DevBuf<float> d_ring, d_carry;
   int ring_len = 0;
   long long blocks_done = 0;
   int reserved_sms = 0;
   // delay memory of the section-8(f) functors: member rows [V][64] and rings [V][stride] per node
   bool has_dmem = false;
-  float* d_dmem = nullptr;
+  DevBuf<float> d_dmem;
   size_t dmem_floats = 0;
   std::vector<unsigned> ring_stride;  // per node, 0 = no ring
 
   // chain scheduler words, all maintained by the kernels themselves (see ChainArgs)
-  unsigned* d_sched = nullptr;
+  DevBuf<unsigned> d_sched;
   int launch_chunks = 1;  // chunks per group of the most recent launch (all slices of one host call agree)
 
   // mix bus partials
-  float* d_partial = nullptr;
-  size_t partial_cap = 0;
+  DevBuf<float> d_partial;
 
   // staging for the host entry point
-  float *d_in = nullptr, *d_out = nullptr, *d_mix = nullptr;
-  size_t in_cap = 0, out_cap = 0, mix_cap = 0;
-  cudaStream_t stream = nullptr, s_h2d = nullptr, s_d2h = nullptr;
-  static constexpr int kMaxHostSlices = 64;
-  cudaEvent_t ev_up[kMaxHostSlices] = {}, ev_k[kMaxHostSlices] = {};
-
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  DevBuf<float> d_in, d_out, d_mix;
   bool timed = false;
   int last_host_slices = 0;  // voice slices of the most recent mlb_graph_process_host call (1 = one launch)
   MapCache maps;
-  // asynchronous mix bus (mlb_graph_set_mix_async): mix_reduce_kernel (and the multi-GPU exchange) run on s_mix,
-  // beside the next call's chain kernel; the per-group partials are double-buffered by call parity
   int mix_async = 0;
-  cudaStream_t s_mix = nullptr;
-  cudaEvent_t ev_main = nullptr, ev_mixdone[4] = {};
   unsigned mix_seq = 0;
   bool mix_pending = false;
   float* partial_cur = nullptr;  // the partial buffer of the call being issued
@@ -1246,8 +1349,9 @@ extern "C" int mlb_graph_create(const mlb_node* nodes, int n_nodes, const int32_
   rc = ensure_init();
   if (rc != MLB_OK) return rc;
 
-  mlb_graph* g = new mlb_graph;
-  ++g_live_handles;
+  std::unique_ptr<mlb_graph> owner(new mlb_graph);
+  mlb_graph* g = owner.get();
+  g->live.arm();
   g->nodes.assign(nodes, nodes + n_nodes);
   g->outs.assign(outs, outs + n_out);
   g->st_off = so;
@@ -1265,24 +1369,13 @@ extern "C" int mlb_graph_create(const mlb_node* nodes, int n_nodes, const int32_
   }
   g->ring_stride.assign(n_nodes, 0u);
 
-  auto cleanup = [&](int code)
-  {
-    mlb_graph_destroy(g);
-    return code;
-  };
   const size_t V = (size_t)n_voices;
-  if (cudaMalloc(&g->d_state, std::max<size_t>(1, lay.n_state_words) * V * 4) != cudaSuccess ||
-      cudaMalloc(&g->d_coef, std::max<size_t>(1, lay.n_coef_words) * V * 4) != cudaSuccess)
-    return cleanup(fail(MLB_ERR_ALLOC, "cudaMalloc of voice state failed: %s",
-                        cudaGetErrorString(cudaGetLastError())));
-  {
-    const size_t n_groups = (V + 31) / 32;
-    // [0] unit counter, [1 + g] finished chunks of group g, [1 + G] finished units, [2 + G] progress base
-    if (cudaMalloc(&g->d_sched, (n_groups + 3) * 4) != cudaSuccess)
-      return cleanup(fail(MLB_ERR_ALLOC, "cudaMalloc of scheduler words failed"));
-    cudaMemset(g->d_sched, 0, (n_groups + 3) * 4);
-  }
-  cudaMemset(g->d_state, 0, std::max<size_t>(1, lay.n_state_words) * V * 4);
+  MLB_TRY(g->d_state.alloc(std::max<size_t>(1, lay.n_state_words) * V * 4, "voice state"));
+  MLB_TRY(g->d_coef.alloc(std::max<size_t>(1, lay.n_coef_words) * V * 4, "voice coefficients"));
+  // [0] unit counter, [1 + g] finished chunks of group g, [1 + G] finished units, [2 + G] progress base
+  MLB_TRY(g->d_sched.alloc(((V + 31) / 32 + 3) * 4, "scheduler words"));
+  CU_CHECK(cudaMemset(g->d_sched.get(), 0, g->d_sched.bytes()));
+  CU_CHECK(cudaMemset(g->d_state.get(), 0, g->d_state.bytes()));
   // state of freshly constructed functors: zeros, except the "idle" markers
   for (int i = 0; i < n_nodes; ++i)
   {
@@ -1294,20 +1387,18 @@ extern "C" int mlb_graph_create(const mlb_node* nodes, int n_nodes, const int32_
     if (nodes[i].op == MLB_OP_TEMPO_LOCK) word = 0, val = 0xBF800000u;    // _omega{-1.f}, F:1481
     if (word < 0) continue;
     std::vector<uint32_t> fill(V, val);
-    cudaMemcpy(g->d_state + (size_t)(so[i] + word) * V, fill.data(), V * 4, cudaMemcpyHostToDevice);
+    CU_CHECK(cudaMemcpy(g->d_state.get() + (size_t)(so[i] + word) * V, fill.data(), V * 4, cudaMemcpyHostToDevice));
   }
-  cudaMemset(g->d_coef, 0, std::max<size_t>(1, lay.n_coef_words) * V * 4);
+  CU_CHECK(cudaMemset(g->d_coef.get(), 0, g->d_coef.bytes()));
   g->h_coef.assign((size_t)lay.n_coef_words * V, 0.f);
-  cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking);
-  cudaStreamCreateWithFlags(&g->s_h2d, cudaStreamNonBlocking);
-  cudaStreamCreateWithFlags(&g->s_d2h, cudaStreamNonBlocking);
+  for (Stream* s : {&g->stream, &g->s_h2d, &g->s_d2h}) MLB_TRY(s->create(cudaStreamNonBlocking));
   for (int i = 0; i < mlb_graph::kMaxHostSlices; ++i)
   {
-    cudaEventCreateWithFlags(&g->ev_up[i], cudaEventDisableTiming);
-    cudaEventCreateWithFlags(&g->ev_k[i], cudaEventDisableTiming);
+    MLB_TRY(g->ev_up[i].create(cudaEventDisableTiming));
+    MLB_TRY(g->ev_k[i].create(cudaEventDisableTiming));
   }
-  cudaEventCreate(&g->ev0);
-  cudaEventCreate(&g->ev1);
+  MLB_TRY(g->ev0.create(cudaEventDefault));
+  MLB_TRY(g->ev1.create(cudaEventDefault));
 
   bool matched = false;
   if (!(flags & MLB_GRAPH_FORCE_GENERIC))
@@ -1324,56 +1415,21 @@ extern "C" int mlb_graph_create(const mlb_node* nodes, int n_nodes, const int32_
   if (!matched)
   {
     g->kind = KIND_GENERIC;
-    rc = build_generic(g);
-    if (rc != MLB_OK) return cleanup(rc);
-    const size_t sync_words = 1 + (size_t)g->n_stages * ((V + 31) / 32);
-    if (cudaMalloc(&g->d_gnodes, sizeof(GNode) * g->gnodes.size()) != cudaSuccess ||
-        cudaMalloc(&g->d_gstages, sizeof(GStage) * g->gstages.size()) != cudaSuccess ||
-        cudaMalloc(&g->d_gsync, sync_words * 4) != cudaSuccess)
-      return cleanup(fail(MLB_ERR_ALLOC, "cudaMalloc of graph program failed"));
-    cudaMemcpy(g->d_gnodes, g->gnodes.data(), sizeof(GNode) * g->gnodes.size(),
-               cudaMemcpyHostToDevice);
-    cudaMemcpy(g->d_gstages, g->gstages.data(), sizeof(GStage) * g->gstages.size(), cudaMemcpyHostToDevice);
-    rc = size_functor_memory(g);
-    if (rc != MLB_OK) return cleanup(rc);
+    MLB_TRY(build_generic(g));
+    MLB_TRY(g->d_gnodes.alloc(sizeof(GNode) * g->gnodes.size(), "graph program"));
+    MLB_TRY(g->d_gstages.alloc(sizeof(GStage) * g->gstages.size(), "graph program"));
+    MLB_TRY(g->d_gsync.alloc((1 + (size_t)g->n_stages * ((V + 31) / 32)) * 4, "graph program"));
+    CU_CHECK(cudaMemcpy(g->d_gnodes.get(), g->gnodes.data(), g->d_gnodes.bytes(), cudaMemcpyHostToDevice));
+    CU_CHECK(cudaMemcpy(g->d_gstages.get(), g->gstages.data(), g->d_gstages.bytes(), cudaMemcpyHostToDevice));
+    MLB_TRY(size_functor_memory(g));
   }
-  *out_graph = g;
+  *out_graph = owner.release();
   return MLB_OK;
 }
 
 extern "C" int mlb_graph_destroy(mlb_graph* g)
 {
-  if (!g) return MLB_OK;
-  cudaFree(g->d_state);
-  cudaFree(g->d_coef);
-  cudaFree(g->d_gnodes);
-  cudaFree(g->d_gstages);
-  cudaFree(g->d_gsync);
-  cudaFree(g->d_chan);
-  cudaFree(g->d_ring);
-  cudaFree(g->d_carry);
-  cudaFree(g->d_dmem);
-  cudaFree(g->d_partial);
-  cudaFree(g->d_sched);
-  cudaFree(g->d_in);
-  cudaFree(g->d_out);
-  cudaFree(g->d_mix);
-  if (g->ev0) cudaEventDestroy(g->ev0);
-  if (g->ev1) cudaEventDestroy(g->ev1);
-  for (int i = 0; i < mlb_graph::kMaxHostSlices; ++i)
-  {
-    if (g->ev_up[i]) cudaEventDestroy(g->ev_up[i]);
-    if (g->ev_k[i]) cudaEventDestroy(g->ev_k[i]);
-  }
-  if (g->s_mix) cudaStreamDestroy(g->s_mix);
-  if (g->ev_main) cudaEventDestroy(g->ev_main);
-  for (cudaEvent_t e : g->ev_mixdone)
-    if (e) cudaEventDestroy(e);
-  if (g->s_h2d) cudaStreamDestroy(g->s_h2d);
-  if (g->s_d2h) cudaStreamDestroy(g->s_d2h);
-  if (g->stream) cudaStreamDestroy(g->stream);
   delete g;
-  --g_live_handles;
   return MLB_OK;
 }
 
@@ -1423,12 +1479,10 @@ static int size_delay_memory(mlb_graph* g)
   while (ring < max_len + MLB_BLOCK) ring <<= 1;
   if (ring != g->ring_len)
   {
-    cudaFree(g->d_ring);
-    cudaFree(g->d_carry);
-    g->d_ring = g->d_carry = nullptr;
-    const size_t ring_bytes = V * 8 * (size_t)ring * 4, carry_bytes = V * 8 * MLB_BLOCK * 4;
-    if (cudaMalloc(&g->d_ring, ring_bytes) != cudaSuccess || cudaMalloc(&g->d_carry, carry_bytes) != cudaSuccess)
-      return fail(MLB_ERR_ALLOC, "cudaMalloc of %zu B delay memory failed", ring_bytes + carry_bytes);
+    g->d_ring.reset();
+    g->d_carry.reset();
+    MLB_TRY(g->d_ring.alloc(V * 8 * (size_t)ring * 4, "delay memory"));
+    MLB_TRY(g->d_carry.alloc(V * 8 * MLB_BLOCK * 4, "delay memory"));
     g->ring_len = ring;
     return mlb_graph_clear_delays(g);
   }
@@ -1491,11 +1545,8 @@ static int size_functor_memory(mlb_graph* g)
     if (g->nodes[i].op == MLB_OP_FEEDBACK_WRITE) row_off[i] = row_off[g->nodes[i].iarg];
   const bool relayout = (total != g->dmem_floats) || (stride != g->ring_stride);
   if (!relayout) return MLB_OK;
-  cudaFree(g->d_dmem);
-  g->d_dmem = nullptr;
   g->dmem_floats = 0;
-  if (cudaMalloc(&g->d_dmem, std::max<unsigned long long>(total, 1) * 4) != cudaSuccess)
-    return fail(MLB_ERR_ALLOC, "cudaMalloc of %llu B delay memory failed", total * 4ull);
+  MLB_TRY(g->d_dmem.alloc(std::max<unsigned long long>(total, 1) * 4, "delay memory"));
   g->dmem_floats = (size_t)total;
   g->ring_stride = stride;
   for (GNode& gn : g->gnodes)
@@ -1505,7 +1556,7 @@ static int size_functor_memory(mlb_graph* g)
     gn.row_off = row_off[gn.src_node];
     gn.ring_off = ring_off[gn.src_node];
   }
-  CU_CHECK(cudaMemcpy(g->d_gnodes, g->gnodes.data(), sizeof(GNode) * g->gnodes.size(), cudaMemcpyHostToDevice));
+  CU_CHECK(cudaMemcpy(g->d_gnodes.get(), g->gnodes.data(), g->d_gnodes.bytes(), cudaMemcpyHostToDevice));
   return mlb_graph_clear_delays(g);
 }
 
@@ -1527,7 +1578,7 @@ extern "C" int mlb_graph_set_coefs(mlb_graph* g, const float* coef_host)
     g->h_coef.swap(old);
     return rc;
   }
-  CU_CHECK(cudaMemcpy(g->d_coef, coef_host, bytes, cudaMemcpyHostToDevice));
+  CU_CHECK(cudaMemcpy(g->d_coef.get(), coef_host, bytes, cudaMemcpyHostToDevice));
   return MLB_OK;
 }
 extern "C" int mlb_graph_set_state(mlb_graph* g, const uint32_t* state_host)
@@ -1535,7 +1586,7 @@ extern "C" int mlb_graph_set_state(mlb_graph* g, const uint32_t* state_host)
   if (!g) return fail(MLB_ERR_INVALID, "null graph");
   if (g->layout.n_state_words == 0) return MLB_OK;
   if (!state_host) return fail(MLB_ERR_INVALID, "null state");
-  CU_CHECK(cudaMemcpy(g->d_state, state_host, (size_t)g->layout.n_state_words * g->V * 4,
+  CU_CHECK(cudaMemcpy(g->d_state.get(), state_host, (size_t)g->layout.n_state_words * g->V * 4,
                       cudaMemcpyHostToDevice));
   return MLB_OK;
 }
@@ -1545,7 +1596,7 @@ extern "C" int mlb_graph_get_state(mlb_graph* g, uint32_t* state_host)
   if (g->layout.n_state_words == 0) return MLB_OK;
   if (!state_host) return fail(MLB_ERR_INVALID, "null state");
   CU_CHECK(cudaDeviceSynchronize());
-  CU_CHECK(cudaMemcpy(state_host, g->d_state, (size_t)g->layout.n_state_words * g->V * 4,
+  CU_CHECK(cudaMemcpy(state_host, g->d_state.get(), (size_t)g->layout.n_state_words * g->V * 4,
                       cudaMemcpyDeviceToHost));
   return MLB_OK;
 }
@@ -1553,19 +1604,19 @@ extern "C" int mlb_graph_clear_delays(mlb_graph* g)
 {
   if (!g) return fail(MLB_ERR_INVALID, "null graph");
   g->blocks_done = 0;
-  if (g->d_ring)
+  if (g->d_ring.get())
   {
-    CU_CHECK(cudaMemset(g->d_ring, 0, (size_t)g->V * 8 * g->ring_len * 4));
-    CU_CHECK(cudaMemset(g->d_carry, 0, (size_t)g->V * 8 * MLB_BLOCK * 4));
+    CU_CHECK(cudaMemset(g->d_ring.get(), 0, (size_t)g->V * 8 * g->ring_len * 4));
+    CU_CHECK(cudaMemset(g->d_carry.get(), 0, (size_t)g->V * 8 * MLB_BLOCK * 4));
   }
-  if (g->d_dmem) CU_CHECK(cudaMemset(g->d_dmem, 0, g->dmem_floats * 4));
+  if (g->d_dmem.get()) CU_CHECK(cudaMemset(g->d_dmem.get(), 0, g->dmem_floats * 4));
   return MLB_OK;
 }
 extern "C" size_t mlb_graph_delay_bytes(const mlb_graph* g)
 {
   if (!g) return 0;
   size_t bytes = g->dmem_floats * 4;
-  if (g->d_ring) bytes += (size_t)g->V * 8 * ((size_t)g->ring_len + MLB_BLOCK) * 4;
+  if (g->d_ring.get()) bytes += (size_t)g->V * 8 * ((size_t)g->ring_len + MLB_BLOCK) * 4;
   return bytes;
 }
 
@@ -1574,20 +1625,22 @@ extern "C" size_t mlb_graph_delay_bytes(const mlb_graph* g)
 
 struct mlb_mixbus
 {
+  // declared first, so released after the exchange buffer (whose cudaFree waits for the device)
+  LiveCount live;
+  static constexpr int kStage = 4;  // calls whose exchange may still be pending on the side stream
+  Event ev_done[kStage], ev_posted;
+  Stream side;                    // completion on a side stream (mlb_mixbus_set_async)
   int rank = 0, world = 1;
   size_t n_floats = 0;   // floats per slot
-  int n_planes_cap = 0;  // flag words per (parity, rank)
-  void* base = nullptr;  // one allocation: xchg [2][world][n_floats] f32, then flags [2][world][n_planes_cap] u32
+  DevBuf<char> base;     // one allocation: xchg [2][world][n_floats] f32, then flags [2][world][flag_planes()] u32
   void* peer_base[kMaxBusRanks] = {};
   bool connected = false;
   unsigned seq = 0;
-  int async = 0;                  // completion on a side stream (mlb_mixbus_set_async)
-  cudaStream_t side = nullptr;
-  static constexpr int kStage = 4;  // calls whose exchange may still be pending on the side stream
-  cudaEvent_t ev_posted = nullptr, ev_done[kStage] = {};
+  int async = 0;
   bool done_pending = false;
+  int flag_planes() const { return (int)(n_floats / MLB_BLOCK); }  // flag words per (parity, rank)
   size_t xchg_bytes() const { return (size_t)2 * world * n_floats * 4; }
-  size_t flag_bytes() const { return (size_t)2 * world * n_planes_cap * 4; }
+  size_t flag_bytes() const { return (size_t)2 * world * flag_planes() * 4; }
   size_t stage_bytes() const { return (size_t)kStage * n_floats * 4; }
   size_t total_bytes() const { return xchg_bytes() + 2 * flag_bytes() + stage_bytes(); }  // slots, flags, acks, staging
 };
@@ -1600,27 +1653,23 @@ extern "C" int mlb_mixbus_create(int rank, int world, size_t max_floats, mlb_mix
     return fail(MLB_ERR_INVALID, "mlb_mixbus_create: need 0 <= rank < world <= %d and max_floats a multiple of 64", kMaxBusRanks);
   int rc = ensure_init();
   if (rc != MLB_OK) return rc;
-  mlb_mixbus* b = new mlb_mixbus;
-  b->rank = rank, b->world = world, b->n_floats = max_floats, b->n_planes_cap = (int)(max_floats / MLB_BLOCK);
-  if (cudaMalloc(&b->base, b->total_bytes()) != cudaSuccess)
-  {
-    delete b;
-    return fail(MLB_ERR_ALLOC, "cudaMalloc of %zu B exchange buffer failed", b->total_bytes());
-  }
-  cudaMemset(b->base, 0, b->total_bytes());
-  cudaDeviceSynchronize();
-  b->peer_base[rank] = b->base;
+  std::unique_ptr<mlb_mixbus> b(new mlb_mixbus);
+  b->live.arm();
+  b->rank = rank, b->world = world, b->n_floats = max_floats;
+  MLB_TRY(b->base.alloc(b->total_bytes(), "exchange buffer"));
+  CU_CHECK(cudaMemset(b->base.get(), 0, b->total_bytes()));
+  CU_CHECK(cudaDeviceSynchronize());
+  b->peer_base[rank] = b->base.get();
   b->connected = (world == 1);
-  cudaStreamCreateWithFlags(&b->side, cudaStreamNonBlocking);
+  MLB_TRY(b->side.create(cudaStreamNonBlocking));
   // The exchange kernel runs BESIDE the next call's chain kernel, whose CTAs need the SM configured for the
   // maximum shared-memory carve-out: a resident CTA that prefers another L1 / shared split keeps the chain CTA
   // off its SM until it has finished.  Ask for the same split.
   cudaFuncSetAttribute((const void*)mixbus_exchange_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
                        (int)cudaSharedmemCarveoutMaxShared);
-  cudaEventCreateWithFlags(&b->ev_posted, cudaEventDisableTiming);
-  for (cudaEvent_t& e : b->ev_done) cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
-  ++g_live_handles;
-  *out = b;
+  MLB_TRY(b->ev_posted.create(cudaEventDisableTiming));
+  for (Event& e : b->ev_done) MLB_TRY(e.create(cudaEventDisableTiming));
+  *out = b.release();
   return MLB_OK;
 }
 extern "C" int mlb_mixbus_handle(mlb_mixbus* b, void* out64)
@@ -1628,7 +1677,7 @@ extern "C" int mlb_mixbus_handle(mlb_mixbus* b, void* out64)
   if (!b || !out64) return fail(MLB_ERR_INVALID, "null argument");
   static_assert(sizeof(cudaIpcMemHandle_t) == 64, "CUDA IPC handle size");
   cudaIpcMemHandle_t h;
-  CU_CHECK(cudaIpcGetMemHandle(&h, b->base));
+  CU_CHECK(cudaIpcGetMemHandle(&h, b->base.get()));
   memcpy(out64, &h, 64);
   return MLB_OK;
 }
@@ -1651,13 +1700,7 @@ extern "C" int mlb_mixbus_destroy(mlb_mixbus* b)
   cudaDeviceSynchronize();
   for (int r = 0; r < b->world; ++r)
     if (r != b->rank && b->peer_base[r]) cudaIpcCloseMemHandle(b->peer_base[r]);
-  cudaFree(b->base);
-  if (b->side) cudaStreamDestroy(b->side);
-  if (b->ev_posted) cudaEventDestroy(b->ev_posted);
-  for (cudaEvent_t e : b->ev_done)
-    if (e) cudaEventDestroy(e);
   delete b;
-  --g_live_handles;
   return MLB_OK;
 }
 extern "C" int mlb_mixbus_set_async(mlb_mixbus* b, int on)
@@ -1673,9 +1716,9 @@ extern "C" int mlb_graph_mix_wait(mlb_graph* g, void* stream)
   if (!g) return fail(MLB_ERR_INVALID, "null graph");
   mlb_mixbus* b = g->bus;
   if (g->mix_async && g->mix_pending)
-    CU_CHECK(cudaStreamWaitEvent((cudaStream_t)stream, g->ev_mixdone[g->mix_seq & 3u], 0));
+    CU_CHECK(cudaStreamWaitEvent((cudaStream_t)stream, g->ev_mixdone[g->mix_seq & 3u].get(), 0));
   if (b && b->async && b->done_pending)
-    CU_CHECK(cudaStreamWaitEvent((cudaStream_t)stream, b->ev_done[b->seq % mlb_mixbus::kStage], 0));
+    CU_CHECK(cudaStreamWaitEvent((cudaStream_t)stream, b->ev_done[b->seq % mlb_mixbus::kStage].get(), 0));
   return MLB_OK;
 }
 extern "C" int mlb_graph_attach_mixbus(mlb_graph* g, mlb_mixbus* b)
@@ -1697,7 +1740,7 @@ static int bus_args(mlb_graph* g, int n_planes, MixBusArgs* a, cudaStream_t stre
                 (size_t)n_planes * MLB_BLOCK);
   a->rank = b->rank, a->world = b->world;
   a->seq = ++b->seq;
-  a->n_floats = (int)b->n_floats, a->n_planes_cap = b->n_planes_cap;
+  a->n_floats = (int)b->n_floats, a->n_planes_cap = b->flag_planes();
   for (int r = 0; r < b->world; ++r)
   {
     a->xchg[r] = (float*)b->peer_base[r];
@@ -1708,9 +1751,9 @@ static int bus_args(mlb_graph* g, int n_planes, MixBusArgs* a, cudaStream_t stre
   if (b->async)
   {
     // staging block of this call; its previous user (four calls ago) must have been exchanged
-    a->stage = (float*)((char*)b->base + b->xchg_bytes() + 2 * b->flag_bytes()) + (size_t)(a->seq % mlb_mixbus::kStage) * b->n_floats;
+    a->stage = (float*)(b->base.get() + b->xchg_bytes() + 2 * b->flag_bytes()) + (size_t)(a->seq % mlb_mixbus::kStage) * b->n_floats;
     if (a->seq > (unsigned)mlb_mixbus::kStage)
-      CU_CHECK(cudaStreamWaitEvent(stream, b->ev_done[a->seq % mlb_mixbus::kStage], 0));
+      CU_CHECK(cudaStreamWaitEvent(stream, b->ev_done[a->seq % mlb_mixbus::kStage].get(), 0));
   }
   return MLB_OK;
 }
@@ -1721,16 +1764,16 @@ static int bus_complete(mlb_graph* g, const MixBusArgs& ba, int n_planes, float*
   if (!b || b->world <= 1 || !b->async) return MLB_OK;
   static const int dbg = env_int("MLB_BUS_DEBUG", 0);  // timing experiments only: 1 = events but no kernel, 2 = nothing
   if (dbg == 2) return MLB_OK;
-  CU_CHECK(cudaEventRecord(b->ev_posted, stream));
-  CU_CHECK(cudaStreamWaitEvent(b->side, b->ev_posted, 0));
+  CU_CHECK(cudaEventRecord(b->ev_posted.get(), stream));
+  CU_CHECK(cudaStreamWaitEvent(b->side.get(), b->ev_posted.get(), 0));
   if (dbg != 1)
   {
     mixbus_exchange_kernel<<<(n_planes + kExchangePlanesPerCta - 1) / kExchangePlanesPerCta,
-                             64 * kExchangePlanesPerCta, 0, b->side>>>(mix_dev, ba, n_planes);
+                             64 * kExchangePlanesPerCta, 0, b->side.get()>>>(mix_dev, ba, n_planes);
     ++g_launches;
     CU_CHECK(cudaGetLastError());
   }
-  CU_CHECK(cudaEventRecord(b->ev_done[ba.seq % mlb_mixbus::kStage], b->side));
+  CU_CHECK(cudaEventRecord(b->ev_done[ba.seq % mlb_mixbus::kStage].get(), b->side.get()));
   b->done_pending = true;
   return MLB_OK;
 }
@@ -1741,34 +1784,16 @@ static int env_int(const char* name, int dflt)
   return (s && *s) ? atoi(s) : dflt;
 }
 
-static int ensure_buf(float** p, size_t* cap, size_t bytes)
-{
-  if (bytes <= *cap) return MLB_OK;
-  cudaFree(*p);
-  *p = nullptr;
-  *cap = 0;
-  if (cudaMalloc(p, bytes) != cudaSuccess) return fail(MLB_ERR_ALLOC, "cudaMalloc of %zu B staging failed", bytes);
-  *cap = bytes;
-  return MLB_OK;
-}
-
 static int ensure_partial(mlb_graph* g, int T, int n_groups)
 {
   // per-group partials followed by the per-chunk scratch of mix_reduce_kernel
   const size_t n_chunks = ((size_t)n_groups + kMixChunkGroups - 1) / kMixChunkGroups;
   const size_t one = (size_t)T * std::max<size_t>(1, g->outs.size()) * ((size_t)n_groups + n_chunks) * MLB_BLOCK * 4;
   const size_t need = one * (g->mix_async ? 2 : 1);  // async: two buffers, alternating by call parity
-  if (need > g->partial_cap)
-  {
-    if (g->mix_pending) cudaStreamSynchronize(g->s_mix);  // nothing may still read the old buffers
-    cudaFree(g->d_partial);
-    g->d_partial = nullptr;
-    g->partial_cap = 0;
-    if (cudaMalloc(&g->d_partial, need) != cudaSuccess)
-      return fail(MLB_ERR_ALLOC, "cudaMalloc of %zu B mix partials failed", need);
-    g->partial_cap = need;
-  }
-  g->partial_cur = g->d_partial;
+  if (need > g->d_partial.bytes() && g->mix_pending)
+    cudaStreamSynchronize(g->s_mix.get());  // nothing may still read the old buffers
+  MLB_TRY(g->d_partial.ensure(need, "mix partials"));
+  g->partial_cur = g->d_partial.get();
   return MLB_OK;
 }
 
@@ -1784,8 +1809,8 @@ static int launch_chain_slice(mlb_graph* g, const float* in_dev, float* out_dev,
   const int n_in = g->layout.n_inputs;
   int rc;
   ChainArgs a = g->cargs;
-  a.state = g->d_state + va;
-  a.coef = g->d_coef + va;
+  a.state = g->d_state.get() + va;
+  a.coef = g->d_coef.get() + va;
   a.mix_partial = want_mix ? g->partial_cur + (size_t)(va / 32) * MLB_BLOCK : nullptr;
   a.V = Vs;
   a.T = T;
@@ -1807,8 +1832,8 @@ static int launch_chain_slice(mlb_graph* g, const float* in_dev, float* out_dev,
     const int S = std::min(std::max(env_int("MLB_TEAM_STAGES", 5), 4), 5);
     a.stages = S;
     a.chunk_blocks = T, a.n_chunks = 1;
-    a.sched = g->d_sched, a.progress = g->d_sched + 1 + va / 32;
-    a.done = g->d_sched + 1 + groups_total, a.base_word = g->d_sched + 2 + groups_total;
+    a.sched = g->d_sched.get(), a.progress = g->d_sched.get() + 1 + va / 32;
+    a.done = g->d_sched.get() + 1 + groups_total, a.base_word = g->d_sched.get() + 2 + groups_total;
     g->launch_chunks = 1;
     const size_t smem = (size_t)S * kBlockBytes + (size_t)S * 8;
     CUtensorMap in_map, out_map;
@@ -1895,10 +1920,10 @@ static int launch_chain_slice(mlb_graph* g, const float* in_dev, float* out_dev,
     n_chunks = std::min(std::max(n_chunks, 1), T);
     a.chunk_blocks = (T + n_chunks - 1) / n_chunks;
     a.n_chunks = (T + a.chunk_blocks - 1) / a.chunk_blocks;
-    a.sched = g->d_sched;
-    a.progress = g->d_sched + 1 + va / 32;
-    a.done = g->d_sched + 1 + groups_total;
-    a.base_word = g->d_sched + 2 + groups_total;
+    a.sched = g->d_sched.get();
+    a.progress = g->d_sched.get() + 1 + va / 32;
+    a.done = g->d_sched.get() + 1 + groups_total;
+    a.base_word = g->d_sched.get() + 2 + groups_total;
     g->launch_chunks = a.n_chunks;
   }
   const size_t smem = (size_t)W * S * stage_bytes + (size_t)W * S * 8;
@@ -1939,7 +1964,7 @@ extern "C" int mlb_graph_process_device(mlb_graph* g, const float* in_dev, float
   if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive");
   if (g->layout.n_inputs > 0 && !in_dev) return fail(MLB_ERR_INVALID, "graph has INPUT nodes but in is null");
   if (g->outs.empty() && (out_dev || mix_dev)) return fail(MLB_ERR_INVALID, "graph has no outputs");
-  if (g->fdn_node >= 0 && !g->d_ring)
+  if (g->fdn_node >= 0 && !g->d_ring.get())
     return fail(MLB_ERR_INVALID, "FDN8 graph: call mlb_graph_set_coefs before processing");
   int rc = ensure_init();
   if (rc != MLB_OK) return rc;
@@ -1955,8 +1980,8 @@ extern "C" int mlb_graph_process_device(mlb_graph* g, const float* in_dev, float
     {
       // this call's partial buffer; its previous user (two calls ago) must have been reduced
       ++g->mix_seq;
-      g->partial_cur = g->d_partial + (size_t)(g->mix_seq & 1u) * (g->partial_cap / 8);
-      if (g->mix_seq > 2u) CU_CHECK(cudaStreamWaitEvent(stream, g->ev_mixdone[(g->mix_seq - 2u) & 3u], 0));
+      g->partial_cur = g->d_partial.get() + (size_t)(g->mix_seq & 1u) * (g->d_partial.bytes() / 8);
+      if (g->mix_seq > 2u) CU_CHECK(cudaStreamWaitEvent(stream, g->ev_mixdone[(g->mix_seq - 2u) & 3u].get(), 0));
     }
   }
 
@@ -1967,7 +1992,7 @@ extern "C" int mlb_graph_process_device(mlb_graph* g, const float* in_dev, float
   if (capturing && (g->fdn_node >= 0 || g->has_dmem || (g->bus && g->bus->world > 1) || (g->mix_async && mix_dev)))
     return fail(MLB_ERR_UNSUPPORTED, "CUDA-graph capture of a process call is supported for graphs without delay "
                                      "memory and without a mix bus (their call counters are kernel arguments)");
-  if (!capturing) cudaEventRecord(g->ev0, stream);
+  if (!capturing) cudaEventRecord(g->ev0.get(), stream);
   if (g->kind == KIND_FUSED)
   {
     rc = launch_chain_slice(g, in_dev, out_dev, mix_dev != nullptr, T, stream, 0, V);
@@ -1979,12 +2004,11 @@ extern "C" int mlb_graph_process_device(mlb_graph* g, const float* in_dev, float
     float* planes = out_dev;
     if (!planes)
     {
-      rc = ensure_buf(&g->d_out, &g->out_cap, (size_t)T * 2 * V * MLB_BLOCK * 4);
-      if (rc != MLB_OK) return rc;
-      planes = g->d_out;
+      MLB_TRY(g->d_out.ensure((size_t)T * 2 * V * MLB_BLOCK * 4, "staging"));
+      planes = g->d_out.get();
     }
-    rc = launch_fm3_fdn8(g->fargs, g->exact, g->d_state, g->d_coef, g->d_ring, g->d_carry, g->ring_len,
-                         g->blocks_done, in_dev, planes, V, T, std::max(1, n_in), stream);
+    rc = launch_fm3_fdn8(g->fargs, g->exact, g->d_state.get(), g->d_coef.get(), g->d_ring.get(), g->d_carry.get(),
+                         g->ring_len, g->blocks_done, in_dev, planes, V, T, std::max(1, n_in), stream);
     if (rc != MLB_OK) return fail(rc, "fdn8 launch failed: %s", cudaGetErrorString(cudaGetLastError()));
     ++g_launches;
     if (mix_dev)
@@ -1998,31 +2022,27 @@ extern "C" int mlb_graph_process_device(mlb_graph* g, const float* in_dev, float
   {
     GenericArgs a;
     memset(&a, 0, sizeof(a));
-    a.nodes = g->d_gnodes;
+    a.nodes = g->d_gnodes.get();
     a.n_nodes = (int)g->gnodes.size();
-    a.state = g->d_state;
-    a.coef = g->d_coef;
+    a.state = g->d_state.get();
+    a.coef = g->d_coef.get();
     a.in = in_dev;
     a.out = out_dev;
     a.mix_partial = mix_dev ? g->partial_cur : nullptr;
     a.V = V, a.T = T, a.n_in = std::max(1, n_in), a.n_out = std::max(1, n_out);
     a.n_groups = n_groups, a.n_slots = g->n_slots;
-    a.fdn_ring = g->d_ring, a.fdn_carry = g->d_carry, a.fdn_ring_len = g->ring_len;
+    a.fdn_ring = g->d_ring.get(), a.fdn_carry = g->d_carry.get(), a.fdn_ring_len = g->ring_len;
     a.blocks_done = g->blocks_done;
-    a.dmem = g->d_dmem;
+    a.dmem = g->d_dmem.get();
     a.scratch_slot = g->scratch_slot;
-    a.stages = g->d_gstages;
+    a.stages = g->d_gstages.get();
     a.n_stages = g->n_stages;
     a.n_chan = g->n_chan;
-    a.sync = g->d_gsync;
-    if (g->n_chan > 0)
-    {
-      rc = ensure_buf(&g->d_chan, &g->chan_cap, (size_t)T * g->n_chan * V * MLB_BLOCK * 4);
-      if (rc != MLB_OK) return rc;
-    }
-    a.chan = g->d_chan;
+    a.sync = g->d_gsync.get();
+    if (g->n_chan > 0) MLB_TRY(g->d_chan.ensure((size_t)T * g->n_chan * V * MLB_BLOCK * 4, "staging"));
+    a.chan = g->d_chan.get();
     const int grid = n_groups * g->n_stages;
-    CU_CHECK(cudaMemsetAsync(g->d_gsync, 0, (1 + (size_t)grid) * 4, stream));
+    CU_CHECK(cudaMemsetAsync(g->d_gsync.get(), 0, (1 + (size_t)grid) * 4, stream));
     const size_t smem = (size_t)g->n_slots * kSlotBytes;
     if (g->exact)
     {
@@ -2040,7 +2060,7 @@ extern "C" int mlb_graph_process_device(mlb_graph* g, const float* in_dev, float
   }
   if (!capturing)
   {
-    cudaEventRecord(g->ev1, stream);
+    cudaEventRecord(g->ev1.get(), stream);
     g->timed = true;
   }
   CU_CHECK(cudaGetLastError());
@@ -2051,9 +2071,9 @@ extern "C" int mlb_graph_process_device(mlb_graph* g, const float* in_dev, float
     cudaStream_t ms = stream;
     if (g->mix_async)
     {
-      CU_CHECK(cudaEventRecord(g->ev_main, stream));
-      CU_CHECK(cudaStreamWaitEvent(g->s_mix, g->ev_main, 0));
-      ms = g->s_mix;
+      CU_CHECK(cudaEventRecord(g->ev_main.get(), stream));
+      CU_CHECK(cudaStreamWaitEvent(g->s_mix.get(), g->ev_main.get(), 0));
+      ms = g->s_mix.get();
     }
     float* scratch = g->partial_cur + (size_t)T * std::max(1, n_out) * n_groups * MLB_BLOCK;
     MixBusArgs ba;
@@ -2068,7 +2088,7 @@ extern "C" int mlb_graph_process_device(mlb_graph* g, const float* in_dev, float
     CU_CHECK(cudaGetLastError());
     if (g->mix_async)
     {
-      CU_CHECK(cudaEventRecord(g->ev_mixdone[g->mix_seq & 3u], ms));
+      CU_CHECK(cudaEventRecord(g->ev_mixdone[g->mix_seq & 3u].get(), ms));
       g->mix_pending = true;
     }
     rc = bus_complete(g, ba, T * std::max(1, n_out), mix_dev, ms);
@@ -2080,13 +2100,13 @@ extern "C" int mlb_graph_process_device(mlb_graph* g, const float* in_dev, float
 extern "C" int mlb_graph_set_mix_async(mlb_graph* g, int on)
 {
   if (!g) return fail(MLB_ERR_INVALID, "null graph");
-  if (g->mix_pending) CU_CHECK(cudaStreamSynchronize(g->s_mix));
+  if (g->mix_pending) CU_CHECK(cudaStreamSynchronize(g->s_mix.get()));
   g->mix_pending = false;
-  if (on && !g->s_mix)
+  if (on)
   {
-    CU_CHECK(cudaStreamCreateWithFlags(&g->s_mix, cudaStreamNonBlocking));
-    CU_CHECK(cudaEventCreateWithFlags(&g->ev_main, cudaEventDisableTiming));
-    for (cudaEvent_t& e : g->ev_mixdone) CU_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    MLB_TRY(g->s_mix.create(cudaStreamNonBlocking));
+    MLB_TRY(g->ev_main.create(cudaEventDisableTiming));
+    for (Event& e : g->ev_mixdone) MLB_TRY(e.create(cudaEventDisableTiming));
   }
   g->mix_async = on ? 1 : 0;
   return MLB_OK;
@@ -2104,10 +2124,10 @@ extern "C" int mlb_graph_process_host(mlb_graph* g, const float* in_host, float*
   const size_t in_bytes = T * n_in * V * MLB_BLOCK * 4, out_bytes = T * n_out * V * MLB_BLOCK * 4;
   const size_t mix_bytes = T * n_out * MLB_BLOCK * 4;
   if (n_in && !in_host) return fail(MLB_ERR_INVALID, "graph has INPUT nodes but in is null");
-  if (n_in && (rc = ensure_buf(&g->d_in, &g->in_cap, in_bytes)) != MLB_OK) return rc;
-  if (out_host && (rc = ensure_buf(&g->d_out, &g->out_cap, out_bytes)) != MLB_OK) return rc;
-  if (mix_host && (rc = ensure_buf(&g->d_mix, &g->mix_cap, mix_bytes)) != MLB_OK) return rc;
-  cudaStream_t s = g->stream;
+  if (n_in) MLB_TRY(g->d_in.ensure(in_bytes, "staging"));
+  if (out_host) MLB_TRY(g->d_out.ensure(out_bytes, "staging"));
+  if (mix_host) MLB_TRY(g->d_mix.ensure(mix_bytes, "staging"));
+  cudaStream_t s = g->stream.get();
   // Large fused banks: pipeline over voice slices so that the H2D copy of slice p+1, the kernel
   // of slice p and the D2H copy of slice p-1 overlap (three streams; PCIe is full duplex).
   // A slice is a strided window [T*n][va:vb][64] of the host planes -> cudaMemcpy2DAsync.
@@ -2126,7 +2146,7 @@ extern "C" int mlb_graph_process_host(mlb_graph* g, const float* in_host, float*
     if (mix_host && (rc = ensure_partial(g, n_blocks, (g->V + 31) / 32)) != MLB_OK) return rc;
     if (mix_host && (rc = mlb_graph_mix_wait(g, s)) != MLB_OK) return rc;  // an asynchronous reduce may still read the partials
     int chunks = 0;
-    cudaEventRecord(g->ev0, s);
+    cudaEventRecord(g->ev0.get(), s);
     g->last_host_slices = 0;
     for (int p = 0, va = 0; va < g->V; ++p, va += per)
     {
@@ -2135,24 +2155,24 @@ extern "C" int mlb_graph_process_host(mlb_graph* g, const float* in_host, float*
       const size_t width = (size_t)(vb - va) * MLB_BLOCK * 4;
       if (n_in)
       {
-        CU_CHECK(cudaMemcpy2DAsync(g->d_in + (size_t)va * MLB_BLOCK, pitch, in_host + (size_t)va * MLB_BLOCK,
-                                   pitch, width, T * n_in, cudaMemcpyHostToDevice, g->s_h2d));
-        CU_CHECK(cudaEventRecord(g->ev_up[p], g->s_h2d));
-        CU_CHECK(cudaStreamWaitEvent(s, g->ev_up[p], 0));
+        CU_CHECK(cudaMemcpy2DAsync(g->d_in.get() + (size_t)va * MLB_BLOCK, pitch, in_host + (size_t)va * MLB_BLOCK,
+                                   pitch, width, T * n_in, cudaMemcpyHostToDevice, g->s_h2d.get()));
+        CU_CHECK(cudaEventRecord(g->ev_up[p].get(), g->s_h2d.get()));
+        CU_CHECK(cudaStreamWaitEvent(s, g->ev_up[p].get(), 0));
       }
-      rc = launch_chain_slice(g, n_in ? g->d_in : nullptr, out_host ? g->d_out : nullptr, mix_host != nullptr,
-                              n_blocks, s, va, vb, chunks);
+      rc = launch_chain_slice(g, n_in ? g->d_in.get() : nullptr, out_host ? g->d_out.get() : nullptr,
+                              mix_host != nullptr, n_blocks, s, va, vb, chunks);
       if (rc != MLB_OK) return rc;
       chunks = g->launch_chunks;
       if (out_host)
       {
-        CU_CHECK(cudaEventRecord(g->ev_k[p], s));
-        CU_CHECK(cudaStreamWaitEvent(g->s_d2h, g->ev_k[p], 0));
-        CU_CHECK(cudaMemcpy2DAsync(out_host + (size_t)va * MLB_BLOCK, pitch, g->d_out + (size_t)va * MLB_BLOCK,
-                                   pitch, width, T * n_out, cudaMemcpyDeviceToHost, g->s_d2h));
+        CU_CHECK(cudaEventRecord(g->ev_k[p].get(), s));
+        CU_CHECK(cudaStreamWaitEvent(g->s_d2h.get(), g->ev_k[p].get(), 0));
+        CU_CHECK(cudaMemcpy2DAsync(out_host + (size_t)va * MLB_BLOCK, pitch, g->d_out.get() + (size_t)va * MLB_BLOCK,
+                                   pitch, width, T * n_out, cudaMemcpyDeviceToHost, g->s_d2h.get()));
       }
     }
-    cudaEventRecord(g->ev1, s);
+    cudaEventRecord(g->ev1.get(), s);
     g->timed = true;
     if (mix_host)
     {
@@ -2162,29 +2182,29 @@ extern "C" int mlb_graph_process_host(mlb_graph* g, const float* in_host, float*
       rc = bus_args(g, (int)(T * std::max<size_t>(1, n_out)), &ba, s);
       if (rc != MLB_OK) return rc;
       mix_reduce_kernel<<<(int)(T * std::max<size_t>(1, n_out)), dim3(MLB_BLOCK, 16), 0, s>>>(g->partial_cur, scratch,
-                                                                                            g->d_mix, n_groups, ba);
-      rc = bus_complete(g, ba, (int)(T * std::max<size_t>(1, n_out)), g->d_mix, s);
+                                                                                            g->d_mix.get(), n_groups, ba);
+      rc = bus_complete(g, ba, (int)(T * std::max<size_t>(1, n_out)), g->d_mix.get(), s);
       if (rc != MLB_OK) return rc;
       rc = mlb_graph_mix_wait(g, s);  // the host entry point returns finished results
       if (rc != MLB_OK) return rc;
       ++g_launches;
       CU_CHECK(cudaGetLastError());
-      CU_CHECK(cudaMemcpyAsync(mix_host, g->d_mix, mix_bytes, cudaMemcpyDeviceToHost, s));
+      CU_CHECK(cudaMemcpyAsync(mix_host, g->d_mix.get(), mix_bytes, cudaMemcpyDeviceToHost, s));
     }
     CU_CHECK(cudaStreamSynchronize(s));
-    CU_CHECK(cudaStreamSynchronize(g->s_d2h));
+    CU_CHECK(cudaStreamSynchronize(g->s_d2h.get()));
     return MLB_OK;
   }
-  if (n_in) CU_CHECK(cudaMemcpyAsync(g->d_in, in_host, in_bytes, cudaMemcpyHostToDevice, s));
-  rc = mlb_graph_process_device(g, n_in ? g->d_in : nullptr, out_host ? g->d_out : nullptr,
-                                mix_host ? g->d_mix : nullptr, n_blocks, s);
+  if (n_in) CU_CHECK(cudaMemcpyAsync(g->d_in.get(), in_host, in_bytes, cudaMemcpyHostToDevice, s));
+  rc = mlb_graph_process_device(g, n_in ? g->d_in.get() : nullptr, out_host ? g->d_out.get() : nullptr,
+                                mix_host ? g->d_mix.get() : nullptr, n_blocks, s);
   if (rc != MLB_OK) return rc;
-  if (out_host) CU_CHECK(cudaMemcpyAsync(out_host, g->d_out, out_bytes, cudaMemcpyDeviceToHost, s));
+  if (out_host) CU_CHECK(cudaMemcpyAsync(out_host, g->d_out.get(), out_bytes, cudaMemcpyDeviceToHost, s));
   if (mix_host)
   {
     rc = mlb_graph_mix_wait(g, s);  // async mix bus: the completion runs on a side stream
     if (rc != MLB_OK) return rc;
-    CU_CHECK(cudaMemcpyAsync(mix_host, g->d_mix, mix_bytes, cudaMemcpyDeviceToHost, s));
+    CU_CHECK(cudaMemcpyAsync(mix_host, g->d_mix.get(), mix_bytes, cudaMemcpyDeviceToHost, s));
   }
   CU_CHECK(cudaStreamSynchronize(s));
   return MLB_OK;
@@ -2196,8 +2216,8 @@ extern "C" int mlb_graph_last_kernel_ms(mlb_graph* g, float* ms)
 {
   if (!g || !ms) return fail(MLB_ERR_INVALID, "null");
   if (!g->timed) return fail(MLB_ERR_INVALID, "no launch recorded yet");
-  CU_CHECK(cudaEventSynchronize(g->ev1));
-  CU_CHECK(cudaEventElapsedTime(ms, g->ev0, g->ev1));
+  CU_CHECK(cudaEventSynchronize(g->ev1.get()));
+  CU_CHECK(cudaEventElapsedTime(ms, g->ev0.get(), g->ev1.get()));
   return MLB_OK;
 }
 
@@ -2288,32 +2308,23 @@ extern "C" int mlb_map_host(int op, const float* x1, const float* x2, const floa
 
 struct mlb_voices
 {
+  // declared first, so released last: the buffers below are freed first, and cudaFree waits for the device
+  LiveCount live;
+  Stream stream;
   int V = 0;
   float sr = 0.f;
   float gl_per = 0.f, gl_dy = 0.f, dr_per = 0.f, dr_dy = 0.f, pc_per = 0.f, pc_dy = 0.f;
   unsigned flags = 0;
-  uint32_t* d_state = nullptr;
-  float* d_coef = nullptr;
-  float* d_grows = nullptr;
-  int32_t* d_main = nullptr;  // MPE: index of each voice's main voice, or -1
-  mlb_voice_events* d_ev = nullptr;
-  float* d_out = nullptr;
-  size_t ev_cap = 0, out_cap = 0;
-  cudaStream_t stream = nullptr;
+  DevBuf<uint32_t> d_state;
+  DevBuf<float> d_coef, d_grows;
+  DevBuf<int32_t> d_main;  // MPE: index of each voice's main voice, or -1
+  DevBuf<mlb_voice_events> d_ev;
+  DevBuf<float> d_out;
 };
 
 extern "C" int mlb_voices_destroy(mlb_voices* vb)
 {
-  if (!vb) return MLB_OK;
-  cudaFree(vb->d_state);
-  cudaFree(vb->d_coef);
-  cudaFree(vb->d_grows);
-  cudaFree(vb->d_main);
-  cudaFree(vb->d_ev);
-  cudaFree(vb->d_out);
-  if (vb->stream) cudaStreamDestroy(vb->stream);
   delete vb;
-  --g_live_handles;
   return MLB_OK;
 }
 
@@ -2328,8 +2339,8 @@ extern "C" int mlb_voices_create(int n_voices, float sample_rate, const int32_t*
   int rc = ensure_init();
   if (rc != MLB_OK) return rc;
   const size_t V = (size_t)n_voices;
-  mlb_voices* vb = new mlb_voices;
-  ++g_live_handles;
+  std::unique_ptr<mlb_voices> vb(new mlb_voices);
+  vb->live.arm();
   vb->V = n_voices;
   vb->sr = sample_rate;
   // the recalc block of the first beginProcess (MLEventsToSignals.cpp:92-113), done once here
@@ -2366,17 +2377,14 @@ extern "C" int mlb_voices_create(int n_voices, float sample_rate, const int32_t*
     co[(size_t)VC_BEND_RANGE * V + v] = pitch_bend[v];
     co[(size_t)VC_VOICE_ROW * V + v] = (float)voice_index[v] - 1;   // :292
   }
-  if (cudaMalloc(&vb->d_state, st.size() * 4) != cudaSuccess || cudaMalloc(&vb->d_coef, co.size() * 4) != cudaSuccess ||
-      cudaMalloc(&vb->d_grows, (size_t)VG_COUNT * V * MLB_BLOCK * 4) != cudaSuccess)
-  {
-    mlb_voices_destroy(vb);
-    return fail(MLB_ERR_ALLOC, "cudaMalloc of voice bank failed");
-  }
-  cudaMemcpy(vb->d_state, st.data(), st.size() * 4, cudaMemcpyHostToDevice);
-  cudaMemcpy(vb->d_coef, co.data(), co.size() * 4, cudaMemcpyHostToDevice);
-  cudaMemset(vb->d_grows, 0, (size_t)VG_COUNT * V * MLB_BLOCK * 4);
-  cudaStreamCreateWithFlags(&vb->stream, cudaStreamNonBlocking);
-  *out = vb;
+  MLB_TRY(vb->d_state.alloc(st.size() * 4, "voice bank"));
+  MLB_TRY(vb->d_coef.alloc(co.size() * 4, "voice bank"));
+  MLB_TRY(vb->d_grows.alloc((size_t)VG_COUNT * V * MLB_BLOCK * 4, "voice bank"));
+  CU_CHECK(cudaMemcpy(vb->d_state.get(), st.data(), st.size() * 4, cudaMemcpyHostToDevice));
+  CU_CHECK(cudaMemcpy(vb->d_coef.get(), co.data(), co.size() * 4, cudaMemcpyHostToDevice));
+  CU_CHECK(cudaMemset(vb->d_grows.get(), 0, vb->d_grows.bytes()));
+  MLB_TRY(vb->stream.create(cudaStreamNonBlocking));
+  *out = vb.release();
   return MLB_OK;
 }
 
@@ -2385,16 +2393,14 @@ extern "C" int mlb_voices_set_main_voices(mlb_voices* vb, const int32_t* main_vo
   if (!vb) return fail(MLB_ERR_INVALID, "null voice bank");
   if (!main_voice)
   {
-    cudaFree(vb->d_main);
-    vb->d_main = nullptr;
+    vb->d_main.reset();
     return MLB_OK;
   }
   for (int v = 0; v < vb->V; ++v)
     if (main_voice[v] >= vb->V || (main_voice[v] >= 0 && main_voice[main_voice[v]] >= 0))
       return fail(MLB_ERR_INVALID, "main_voice[%d] = %d is not a main voice of this bank", v, main_voice[v]);
-  if (!vb->d_main && cudaMalloc(&vb->d_main, (size_t)vb->V * 4) != cudaSuccess)
-    return fail(MLB_ERR_ALLOC, "cudaMalloc of main-voice table failed");
-  CU_CHECK(cudaMemcpy(vb->d_main, main_voice, (size_t)vb->V * 4, cudaMemcpyHostToDevice));
+  MLB_TRY(vb->d_main.ensure((size_t)vb->V * 4, "main-voice table"));
+  CU_CHECK(cudaMemcpy(vb->d_main.get(), main_voice, (size_t)vb->V * 4, cudaMemcpyHostToDevice));
   return MLB_OK;
 }
 
@@ -2406,9 +2412,9 @@ extern "C" int mlb_voices_process_device(mlb_voices* vb, const mlb_voice_events*
   VoiceArgs a;
   a.ev = events_dev;
   a.out = out_dev;
-  a.state = vb->d_state;
-  a.coef = vb->d_coef;
-  a.grows = vb->d_grows;
+  a.state = vb->d_state.get();
+  a.coef = vb->d_coef.get();
+  a.grows = vb->d_grows.get();
   a.V = vb->V, a.T = n_blocks;
   a.row_mask = row_mask & 0xFFu;
   a.sr = vb->sr;
@@ -2434,11 +2440,11 @@ extern "C" int mlb_voices_process_device(mlb_voices* vb, const mlb_voice_events*
     voice_bank_kernel<false><<<(n_warps + wpc - 1) / wpc, 32 * wpc, smem, (cudaStream_t)stream>>>(a);
   ++g_launches;
   CU_CHECK(cudaGetLastError());
-  if (vb->d_main && (a.row_mask & 0x79u))  // MPE: add the main voices' pitch / z / x / y / mod rows
+  if (vb->d_main.get() && (a.row_mask & 0x79u))  // MPE: add the main voices' pitch / z / x / y / mod rows
   {
     const size_t n4 = (size_t)n_blocks * vb->V * 16;
     const int grid = (int)std::min<size_t>((n4 + 255) / 256, (size_t)g_sm_count * 16);
-    voice_mpe_add_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(out_dev, vb->d_main, vb->V, n_blocks, a.row_mask);
+    voice_mpe_add_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(out_dev, vb->d_main.get(), vb->V, n_blocks, a.row_mask);
     ++g_launches;
     CU_CHECK(cudaGetLastError());
   }
@@ -2454,23 +2460,21 @@ extern "C" int mlb_voices_process_host(mlb_voices* vb, const mlb_voice_events* e
   if (row_mask && !out_host) return fail(MLB_ERR_INVALID, "out is null");
   const size_t V = (size_t)vb->V, T = (size_t)n_blocks;
   const size_t ev_bytes = T * V * sizeof(mlb_voice_events), out_bytes = T * MLB_VOICE_ROWS * V * MLB_BLOCK * 4;
-  int rc = ensure_buf(reinterpret_cast<float**>(&vb->d_ev), &vb->ev_cap, ev_bytes);
-  if (rc != MLB_OK) return rc;
-  rc = ensure_buf(&vb->d_out, &vb->out_cap, out_bytes);
-  if (rc != MLB_OK) return rc;
-  cudaStream_t s = vb->stream;
-  CU_CHECK(cudaMemcpyAsync(vb->d_ev, events_host, ev_bytes, cudaMemcpyHostToDevice, s));
-  rc = mlb_voices_process_device(vb, vb->d_ev, vb->d_out, n_blocks, row_mask, s);
+  MLB_TRY(vb->d_ev.ensure(ev_bytes, "staging"));
+  MLB_TRY(vb->d_out.ensure(out_bytes, "staging"));
+  cudaStream_t s = vb->stream.get();
+  CU_CHECK(cudaMemcpyAsync(vb->d_ev.get(), events_host, ev_bytes, cudaMemcpyHostToDevice, s));
+  int rc = mlb_voices_process_device(vb, vb->d_ev.get(), vb->d_out.get(), n_blocks, row_mask, s);
   if (rc != MLB_OK) return rc;
   const size_t plane = V * MLB_BLOCK * 4;
   if (row_mask == 0xFFu)
-    CU_CHECK(cudaMemcpyAsync(out_host, vb->d_out, out_bytes, cudaMemcpyDeviceToHost, s));
+    CU_CHECK(cudaMemcpyAsync(out_host, vb->d_out.get(), out_bytes, cudaMemcpyDeviceToHost, s));
   else
     for (size_t t = 0; t < T; ++t)
       for (int r = 0; r < MLB_VOICE_ROWS; ++r)
         if (row_mask & (1u << r))
           CU_CHECK(cudaMemcpyAsync(reinterpret_cast<char*>(out_host) + (t * MLB_VOICE_ROWS + r) * plane,
-                                   reinterpret_cast<char*>(vb->d_out) + (t * MLB_VOICE_ROWS + r) * plane, plane,
+                                   reinterpret_cast<char*>(vb->d_out.get()) + (t * MLB_VOICE_ROWS + r) * plane, plane,
                                    cudaMemcpyDeviceToHost, s));
   CU_CHECK(cudaStreamSynchronize(s));
   return MLB_OK;
@@ -2525,37 +2529,35 @@ static int synth_pipeline(mlb_voices* vb, mlb_graph* g, const mlb_voice_events* 
                           RunChunk run_chunk)
 {
   const size_t V = (size_t)g->V, T = (size_t)n_blocks;
-  int rc;
-  if ((rc = ensure_buf(reinterpret_cast<float**>(&vb->d_ev), &vb->ev_cap, T * V * sizeof(mlb_voice_events))) != MLB_OK)
-    return rc;
-  if ((rc = ensure_buf(&vb->d_out, &vb->out_cap, (size_t)Tc * MLB_VOICE_ROWS * V * MLB_BLOCK * 4)) != MLB_OK) return rc;
+  MLB_TRY(vb->d_ev.ensure(T * V * sizeof(mlb_voice_events), "staging"));
+  MLB_TRY(vb->d_out.ensure((size_t)Tc * MLB_VOICE_ROWS * V * MLB_BLOCK * 4, "staging"));
   const int saved_inputs = g->layout.n_inputs;
   g->layout.n_inputs = MLB_VOICE_ROWS;
-  cudaStream_t s = g->stream;
-  int p = 0;
+  cudaStream_t s = g->stream.get();
+  int rc = MLB_OK, p = 0;
   for (size_t t0 = 0; t0 < T && rc == MLB_OK; t0 += (size_t)Tc, ++p)
   {
     const int tc = (int)std::min<size_t>((size_t)Tc, T - t0);
-    cudaError_t ce = cudaMemcpyAsync(vb->d_ev + t0 * V, events_host + t0 * V, (size_t)tc * V * sizeof(mlb_voice_events),
-                                     cudaMemcpyHostToDevice, g->s_h2d);
-    if (ce == cudaSuccess) ce = cudaEventRecord(g->ev_up[p], g->s_h2d);
-    if (ce == cudaSuccess) ce = cudaStreamWaitEvent(s, g->ev_up[p], 0);
+    cudaError_t ce = cudaMemcpyAsync(vb->d_ev.get() + t0 * V, events_host + t0 * V,
+                                     (size_t)tc * V * sizeof(mlb_voice_events), cudaMemcpyHostToDevice, g->s_h2d.get());
+    if (ce == cudaSuccess) ce = cudaEventRecord(g->ev_up[p].get(), g->s_h2d.get());
+    if (ce == cudaSuccess) ce = cudaStreamWaitEvent(s, g->ev_up[p].get(), 0);
     if (ce != cudaSuccess)
     {
       rc = fail(MLB_ERR_CUDA, "events H2D: %s", cudaGetErrorString(ce));
       break;
     }
-    rc = mlb_voices_process_device(vb, vb->d_ev + t0 * V, vb->d_out, tc, row_mask, s);
+    rc = mlb_voices_process_device(vb, vb->d_ev.get() + t0 * V, vb->d_out.get(), tc, row_mask, s);
     if (rc != MLB_OK) break;
     rc = run_chunk(t0, tc, s);
     if (rc != MLB_OK) break;
     if (down_host)
     {
-      ce = cudaEventRecord(g->ev_k[p], s);
-      if (ce == cudaSuccess) ce = cudaStreamWaitEvent(g->s_d2h, g->ev_k[p], 0);
+      ce = cudaEventRecord(g->ev_k[p].get(), s);
+      if (ce == cudaSuccess) ce = cudaStreamWaitEvent(g->s_d2h.get(), g->ev_k[p].get(), 0);
       if (ce == cudaSuccess)
         ce = cudaMemcpyAsync(down_host + t0 * down_per_block, down_dev + t0 * down_per_block,
-                             (size_t)tc * down_per_block * 4, cudaMemcpyDeviceToHost, g->s_d2h);
+                             (size_t)tc * down_per_block * 4, cudaMemcpyDeviceToHost, g->s_d2h.get());
       if (ce != cudaSuccess) rc = fail(MLB_ERR_CUDA, "rows D2H: %s", cudaGetErrorString(ce));
     }
   }
@@ -2567,8 +2569,8 @@ static int synth_pipeline(mlb_voices* vb, mlb_graph* g, const mlb_voice_events* 
 // Drain all three streams whatever happened: nothing may still touch the caller's buffers on return.
 static int synth_drain(mlb_graph* g, int rc)
 {
-  cudaStreamSynchronize(g->s_h2d);
-  cudaError_t e1 = cudaStreamSynchronize(g->stream), e2 = cudaStreamSynchronize(g->s_d2h);
+  cudaStreamSynchronize(g->s_h2d.get());
+  cudaError_t e1 = cudaStreamSynchronize(g->stream.get()), e2 = cudaStreamSynchronize(g->s_d2h.get());
   if (rc == MLB_OK && (e1 != cudaSuccess || e2 != cudaSuccess))
     rc = fail(MLB_ERR_CUDA, "synth pipeline: %s", cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
   return rc;
@@ -2584,20 +2586,20 @@ extern "C" int mlb_synth_process_host(mlb_voices* vb, mlb_graph* g, const mlb_vo
   if ((rc = ensure_init()) != MLB_OK) return rc;
   const size_t V = (size_t)g->V, T = (size_t)n_blocks, n_out = g->outs.size();
   const int Tc = synth_chunk_blocks(g, n_blocks);
-  if (out_host && (rc = ensure_buf(&g->d_out, &g->out_cap, T * n_out * V * MLB_BLOCK * 4)) != MLB_OK) return rc;
-  if (mix_host && (rc = ensure_buf(&g->d_mix, &g->mix_cap, T * n_out * MLB_BLOCK * 4)) != MLB_OK) return rc;
-  rc = synth_pipeline(vb, g, events_host, n_blocks, row_mask, Tc, g->d_out, out_host, n_out * V * MLB_BLOCK,
+  if (out_host) MLB_TRY(g->d_out.ensure(T * n_out * V * MLB_BLOCK * 4, "staging"));
+  if (mix_host) MLB_TRY(g->d_mix.ensure(T * n_out * MLB_BLOCK * 4, "staging"));
+  rc = synth_pipeline(vb, g, events_host, n_blocks, row_mask, Tc, g->d_out.get(), out_host, n_out * V * MLB_BLOCK,
                       [&](size_t t0, int tc, cudaStream_t s)
                       {
-                        return mlb_graph_process_device(g, vb->d_out,
-                                                        out_host ? g->d_out + t0 * n_out * V * MLB_BLOCK : nullptr,
-                                                        mix_host ? g->d_mix + t0 * n_out * MLB_BLOCK : nullptr, tc, s);
+                        float* out = out_host ? g->d_out.get() + t0 * n_out * V * MLB_BLOCK : nullptr;
+                        float* mix = mix_host ? g->d_mix.get() + t0 * n_out * MLB_BLOCK : nullptr;
+                        return mlb_graph_process_device(g, vb->d_out.get(), out, mix, tc, s);
                       });
   if (rc == MLB_OK && mix_host)
   {
-    rc = mlb_graph_mix_wait(g, g->stream);
-    if (rc == MLB_OK &&
-        cudaMemcpyAsync(mix_host, g->d_mix, T * n_out * MLB_BLOCK * 4, cudaMemcpyDeviceToHost, g->stream) != cudaSuccess)
+    rc = mlb_graph_mix_wait(g, g->stream.get());
+    if (rc == MLB_OK && cudaMemcpyAsync(mix_host, g->d_mix.get(), T * n_out * MLB_BLOCK * 4, cudaMemcpyDeviceToHost,
+                                        g->stream.get()) != cudaSuccess)
       rc = fail(MLB_ERR_CUDA, "mix D2H failed");
   }
   return synth_drain(g, rc);
@@ -2608,19 +2610,15 @@ extern "C" int mlb_synth_process_host(mlb_voices* vb, mlb_graph* g, const mlb_vo
 
 struct mlb_buses
 {
+  LiveCount live;
   int V = 0, G = 0;
-  int32_t* d_table = nullptr;  // [2][G]: first voice, voice count
-  float* d_out = nullptr;      // bus rows of mlb_synth_process_buses_host, [T][n_out][G][64]
-  size_t out_cap = 0;
+  DevBuf<int32_t> d_table;  // [2][G]: first voice, voice count
+  DevBuf<float> d_out;      // bus rows of mlb_synth_process_buses_host, [T][n_out][G][64]
 };
 
 extern "C" int mlb_buses_destroy(mlb_buses* b)
 {
-  if (!b) return MLB_OK;
-  cudaFree(b->d_table);
-  cudaFree(b->d_out);
   delete b;
-  --g_live_handles;
   return MLB_OK;
 }
 
@@ -2638,22 +2636,15 @@ extern "C" int mlb_buses_create(int n_voices, int n_buses, const int32_t* first_
                   first_voice[g], voice_count[g], n_voices);
   int rc = ensure_init();
   if (rc != MLB_OK) return rc;
-  mlb_buses* b = new mlb_buses;
-  ++g_live_handles;
+  std::unique_ptr<mlb_buses> b(new mlb_buses);
+  b->live.arm();
   b->V = n_voices, b->G = n_buses;
   const size_t bytes = (size_t)n_buses * sizeof(int32_t);
-  if (cudaMalloc(&b->d_table, 2 * bytes) != cudaSuccess)
-  {
-    mlb_buses_destroy(b);
-    return fail(MLB_ERR_ALLOC, "cudaMalloc of bus layout failed");
-  }
-  if (cudaMemcpy(b->d_table, first_voice, bytes, cudaMemcpyHostToDevice) != cudaSuccess ||
-      cudaMemcpy(b->d_table + n_buses, voice_count, bytes, cudaMemcpyHostToDevice) != cudaSuccess)
-  {
-    mlb_buses_destroy(b);
+  MLB_TRY(b->d_table.alloc(2 * bytes, "bus layout"));
+  if (cudaMemcpy(b->d_table.get(), first_voice, bytes, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy(b->d_table.get() + n_buses, voice_count, bytes, cudaMemcpyHostToDevice) != cudaSuccess)
     return fail(MLB_ERR_CUDA, "upload of bus layout failed");
-  }
-  *out = b;
+  *out = b.release();
   return MLB_OK;
 }
 
@@ -2664,7 +2655,7 @@ extern "C" int mlb_buses_sum_device(mlb_buses* b, const float* rows_dev, float* 
   if (n_planes <= 0) return fail(MLB_ERR_INVALID, "n_planes must be positive (got %d)", n_planes);
   if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive (got %d)", n_blocks);
   BusArgs a;
-  a.rows = rows_dev, a.bus = bus_dev, a.first = b->d_table, a.count = b->d_table + b->G;
+  a.rows = rows_dev, a.bus = bus_dev, a.first = b->d_table.get(), a.count = b->d_table.get() + b->G;
   a.V = b->V, a.G = b->G;
   a.n_items = (long long)n_blocks * n_planes * b->G;
   const long long grid = (a.n_items + kBusWarps - 1) / kBusWarps;
@@ -2689,15 +2680,15 @@ extern "C" int mlb_synth_process_buses_host(mlb_voices* vb, mlb_graph* g, mlb_bu
   if ((rc = ensure_init()) != MLB_OK) return rc;
   const size_t V = (size_t)g->V, T = (size_t)n_blocks, n_out = g->outs.size(), G = (size_t)b->G;
   const int Tc = synth_chunk_blocks(g, n_blocks);
-  if ((rc = ensure_buf(&g->d_out, &g->out_cap, (size_t)Tc * n_out * V * MLB_BLOCK * 4)) != MLB_OK) return rc;
-  if ((rc = ensure_buf(&b->d_out, &b->out_cap, T * n_out * G * MLB_BLOCK * 4)) != MLB_OK) return rc;
-  rc = synth_pipeline(vb, g, events_host, n_blocks, row_mask, Tc, b->d_out, bus_host, n_out * G * MLB_BLOCK,
+  MLB_TRY(g->d_out.ensure((size_t)Tc * n_out * V * MLB_BLOCK * 4, "staging"));
+  MLB_TRY(b->d_out.ensure(T * n_out * G * MLB_BLOCK * 4, "staging"));
+  rc = synth_pipeline(vb, g, events_host, n_blocks, row_mask, Tc, b->d_out.get(), bus_host, n_out * G * MLB_BLOCK,
                       [&](size_t t0, int tc, cudaStream_t s)
                       {
-                        int r = mlb_graph_process_device(g, vb->d_out, g->d_out, nullptr, tc, s);
+                        int r = mlb_graph_process_device(g, vb->d_out.get(), g->d_out.get(), nullptr, tc, s);
                         if (r != MLB_OK) return r;
-                        return mlb_buses_sum_device(b, g->d_out, b->d_out + t0 * n_out * G * MLB_BLOCK, (int)n_out, tc,
-                                                    s);
+                        return mlb_buses_sum_device(b, g->d_out.get(), b->d_out.get() + t0 * n_out * G * MLB_BLOCK,
+                                                    (int)n_out, tc, s);
                       });
   return synth_drain(g, rc);
 }
@@ -2707,33 +2698,26 @@ extern "C" int mlb_synth_process_buses_host(mlb_voices* vb, mlb_graph* g, mlb_bu
 
 struct mlb_resampler
 {
+  // declared first, so released last: the buffers below are freed first, and cudaFree waits for the device
+  LiveCount live;
+  Stream stream;
   int dir = 0, oct = 0, V = 0;
   unsigned counter = 0;
-  uint32_t* d_state = nullptr;
-  float* d_buf = nullptr;
-  float *d_in = nullptr, *d_out = nullptr;
-  size_t in_cap = 0, out_cap = 0;
-  cudaStream_t stream = nullptr;
+  DevBuf<uint32_t> d_state;
+  DevBuf<float> d_buf, d_in, d_out;
 };
 
 extern "C" int mlb_resampler_destroy(mlb_resampler* r)
 {
-  if (!r) return MLB_OK;
-  cudaFree(r->d_state);
-  cudaFree(r->d_buf);
-  cudaFree(r->d_in);
-  cudaFree(r->d_out);
-  if (r->stream) cudaStreamDestroy(r->stream);
   delete r;
-  --g_live_handles;
   return MLB_OK;
 }
 extern "C" int mlb_resampler_clear(mlb_resampler* r)
 {
   if (!r) return fail(MLB_ERR_INVALID, "null resampler");
   r->counter = 0;
-  CU_CHECK(cudaMemset(r->d_state, 0, (size_t)r->oct * 9 * r->V * 4));
-  if (r->d_buf) CU_CHECK(cudaMemset(r->d_buf, 0, (size_t)(2 * r->oct + 1) * r->V * MLB_BLOCK * 4));
+  CU_CHECK(cudaMemset(r->d_state.get(), 0, r->d_state.bytes()));
+  if (r->d_buf.get()) CU_CHECK(cudaMemset(r->d_buf.get(), 0, r->d_buf.bytes()));
   return MLB_OK;
 }
 extern "C" int mlb_resampler_create(int direction, int octaves, int n_voices, mlb_resampler** out)
@@ -2744,25 +2728,15 @@ extern "C" int mlb_resampler_create(int direction, int octaves, int n_voices, ml
     return fail(MLB_ERR_INVALID, "bad argument (direction %d, octaves %d, voices %d)", direction, octaves, n_voices);
   int rc = ensure_init();
   if (rc != MLB_OK) return rc;
-  mlb_resampler* r = new mlb_resampler;
-  ++g_live_handles;
+  std::unique_ptr<mlb_resampler> r(new mlb_resampler);
+  r->live.arm();
   r->dir = direction, r->oct = octaves, r->V = n_voices;
-  bool ok = cudaMalloc(&r->d_state, (size_t)octaves * 9 * n_voices * 4) == cudaSuccess;
-  if (ok && direction == MLB_RESAMPLE_DOWN)
-    ok = cudaMalloc(&r->d_buf, (size_t)(2 * octaves + 1) * n_voices * MLB_BLOCK * 4) == cudaSuccess;
-  if (!ok)
-  {
-    mlb_resampler_destroy(r);
-    return fail(MLB_ERR_ALLOC, "cudaMalloc of resampler state failed");
-  }
-  cudaStreamCreateWithFlags(&r->stream, cudaStreamNonBlocking);
-  rc = mlb_resampler_clear(r);
-  if (rc != MLB_OK)
-  {
-    mlb_resampler_destroy(r);
-    return rc;
-  }
-  *out = r;
+  MLB_TRY(r->d_state.alloc((size_t)octaves * 9 * n_voices * 4, "resampler state"));
+  if (direction == MLB_RESAMPLE_DOWN)
+    MLB_TRY(r->d_buf.alloc((size_t)(2 * octaves + 1) * n_voices * MLB_BLOCK * 4, "resampler state"));
+  MLB_TRY(r->stream.create(cudaStreamNonBlocking));
+  MLB_TRY(mlb_resampler_clear(r.get()));
+  *out = r.release();
   return MLB_OK;
 }
 static int resampler_out_blocks(const mlb_resampler* r, int n_in)
@@ -2778,7 +2752,7 @@ extern "C" int mlb_resampler_process_device(mlb_resampler* r, const float* in_de
   const int n_out = resampler_out_blocks(r, n_blocks_in);
   if (n_out > 0 && !out_dev) return fail(MLB_ERR_INVALID, "out is null");
   ResampleArgs a;
-  a.in = in_dev, a.out = out_dev, a.state = r->d_state, a.buf = r->d_buf;
+  a.in = in_dev, a.out = out_dev, a.state = r->d_state.get(), a.buf = r->d_buf.get();
   a.V = r->V, a.T = n_blocks_in, a.oct = r->oct, a.counter = r->counter;
   const int grid = (r->V + 127) / 128;
   if (r->dir == MLB_RESAMPLE_UP)
@@ -2801,15 +2775,12 @@ extern "C" int mlb_resampler_process_host(mlb_resampler* r, const float* in_host
   const size_t row = (size_t)r->V * MLB_BLOCK * 4;
   const int n_out = resampler_out_blocks(r, n_blocks_in);
   if (n_out > 0 && !out_host) return fail(MLB_ERR_INVALID, "out is null");
-  int rc = ensure_buf(&r->d_in, &r->in_cap, (size_t)n_blocks_in * row);
-  if (rc != MLB_OK) return rc;
-  rc = ensure_buf(&r->d_out, &r->out_cap, std::max<size_t>(1, (size_t)n_out) * row);
-  if (rc != MLB_OK) return rc;
-  cudaStream_t s = r->stream;
-  CU_CHECK(cudaMemcpyAsync(r->d_in, in_host, (size_t)n_blocks_in * row, cudaMemcpyHostToDevice, s));
-  rc = mlb_resampler_process_device(r, r->d_in, r->d_out, n_blocks_in, n_blocks_out, s);
-  if (rc != MLB_OK) return rc;
-  if (n_out > 0) CU_CHECK(cudaMemcpyAsync(out_host, r->d_out, (size_t)n_out * row, cudaMemcpyDeviceToHost, s));
+  MLB_TRY(r->d_in.ensure((size_t)n_blocks_in * row, "staging"));
+  MLB_TRY(r->d_out.ensure(std::max<size_t>(1, (size_t)n_out) * row, "staging"));
+  cudaStream_t s = r->stream.get();
+  CU_CHECK(cudaMemcpyAsync(r->d_in.get(), in_host, (size_t)n_blocks_in * row, cudaMemcpyHostToDevice, s));
+  MLB_TRY(mlb_resampler_process_device(r, r->d_in.get(), r->d_out.get(), n_blocks_in, n_blocks_out, s));
+  if (n_out > 0) CU_CHECK(cudaMemcpyAsync(out_host, r->d_out.get(), (size_t)n_out * row, cudaMemcpyDeviceToHost, s));
   CU_CHECK(cudaStreamSynchronize(s));
   return MLB_OK;
 }
@@ -2819,32 +2790,27 @@ extern "C" int mlb_resampler_process_host(mlb_resampler* r, const float* in_host
 
 struct mlb_fdtd
 {
+  // declared first, so released last: the buffers below are freed first, and cudaFree waits for the device
+  LiveCount live;
+  Stream stream;
   int V = 0, in_planes = 0, excite = 0, freq = 0;
   unsigned flags = 0;
   float sample_rate = 0.f;
-  float* d_state = nullptr;  // [V][2][16][16]
-  float *d_in = nullptr, *d_out = nullptr;
-  size_t in_cap = 0, out_cap = 0;
-  cudaStream_t stream = nullptr;
+  DevBuf<float> d_state;  // [V][2][16][16]
+  DevBuf<float> d_in, d_out;
 };
 
 static size_t fdtd_state_bytes(const mlb_fdtd* f) { return (size_t)f->V * 2 * kFdtdCells * sizeof(float); }
 
 extern "C" int mlb_fdtd_destroy(mlb_fdtd* f)
 {
-  if (!f) return MLB_OK;
-  cudaFree(f->d_state);
-  cudaFree(f->d_in);
-  cudaFree(f->d_out);
-  if (f->stream) cudaStreamDestroy(f->stream);
   delete f;
-  --g_live_handles;
   return MLB_OK;
 }
 extern "C" int mlb_fdtd_clear(mlb_fdtd* f)
 {
   if (!f) return fail(MLB_ERR_INVALID, "null FDTD bank");
-  CU_CHECK(cudaMemset(f->d_state, 0, fdtd_state_bytes(f)));
+  CU_CHECK(cudaMemset(f->d_state.get(), 0, fdtd_state_bytes(f)));
   CU_CHECK(cudaDeviceSynchronize());
   return MLB_OK;
 }
@@ -2862,37 +2828,28 @@ extern "C" int mlb_fdtd_create(int n_instances, float sample_rate, int in_planes
   if (flags & ~MLB_FDTD_FTZ) return fail(MLB_ERR_INVALID, "unknown flags 0x%x", flags);
   int rc = ensure_init();
   if (rc != MLB_OK) return rc;
-  mlb_fdtd* f = new mlb_fdtd;
-  ++g_live_handles;
+  std::unique_ptr<mlb_fdtd> f(new mlb_fdtd);
+  f->live.arm();
   f->V = n_instances, f->in_planes = in_planes, f->excite = excite_plane, f->freq = freq_plane;
   f->flags = flags, f->sample_rate = sample_rate;
-  if (cudaMalloc(&f->d_state, fdtd_state_bytes(f)) != cudaSuccess)
-  {
-    mlb_fdtd_destroy(f);
-    return fail(MLB_ERR_ALLOC, "cudaMalloc of FDTD state failed");
-  }
-  cudaStreamCreateWithFlags(&f->stream, cudaStreamNonBlocking);
-  rc = mlb_fdtd_clear(f);
-  if (rc != MLB_OK)
-  {
-    mlb_fdtd_destroy(f);
-    return rc;
-  }
-  *out = f;
+  MLB_TRY(f->d_state.alloc(fdtd_state_bytes(f.get()), "FDTD state"));
+  MLB_TRY(f->stream.create(cudaStreamNonBlocking));
+  MLB_TRY(mlb_fdtd_clear(f.get()));
+  *out = f.release();
   return MLB_OK;
 }
 extern "C" int mlb_fdtd_get_state(mlb_fdtd* f, float* host)
 {
   if (!f || !host) return fail(MLB_ERR_INVALID, "null argument");
   CU_CHECK(cudaDeviceSynchronize());
-  CU_CHECK(cudaMemcpy(host, f->d_state, fdtd_state_bytes(f), cudaMemcpyDeviceToHost));
+  CU_CHECK(cudaMemcpy(host, f->d_state.get(), fdtd_state_bytes(f), cudaMemcpyDeviceToHost));
   return MLB_OK;
 }
 extern "C" int mlb_fdtd_set_state(mlb_fdtd* f, const float* host)
 {
   if (!f || !host) return fail(MLB_ERR_INVALID, "null argument");
   CU_CHECK(cudaDeviceSynchronize());
-  CU_CHECK(cudaMemcpy(f->d_state, host, fdtd_state_bytes(f), cudaMemcpyHostToDevice));
+  CU_CHECK(cudaMemcpy(f->d_state.get(), host, fdtd_state_bytes(f), cudaMemcpyHostToDevice));
   return MLB_OK;
 }
 extern "C" int mlb_fdtd_process_device(mlb_fdtd* f, const float* in_dev, float* out_dev, int n_blocks, void* stream)
@@ -2900,7 +2857,7 @@ extern "C" int mlb_fdtd_process_device(mlb_fdtd* f, const float* in_dev, float* 
   if (!f || !in_dev || !out_dev) return fail(MLB_ERR_INVALID, "null argument");
   if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive (got %d)", n_blocks);
   FdtdArgs a;
-  a.in = in_dev, a.out = out_dev, a.state = f->d_state;
+  a.in = in_dev, a.out = out_dev, a.state = f->d_state.get();
   a.V = f->V, a.T = n_blocks, a.in_planes = f->in_planes, a.excite_plane = f->excite, a.freq_plane = f->freq;
   // the example's constants (fdtd.cpp:23, 79, 89, 100-101, 118), rounded on the host as its compiler does
   a.k_size = sqrtf((float)(kFdtdN * kFdtdN) + (float)(kFdtdN * kFdtdN));
@@ -2924,15 +2881,12 @@ extern "C" int mlb_fdtd_process_host(mlb_fdtd* f, const float* in_host, float* o
   if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive (got %d)", n_blocks);
   const size_t row = (size_t)f->V * MLB_BLOCK * sizeof(float);
   const size_t in_bytes = (size_t)n_blocks * f->in_planes * row, out_bytes = (size_t)n_blocks * 2 * row;
-  int rc = ensure_buf(&f->d_in, &f->in_cap, in_bytes);
-  if (rc != MLB_OK) return rc;
-  rc = ensure_buf(&f->d_out, &f->out_cap, out_bytes);
-  if (rc != MLB_OK) return rc;
-  cudaStream_t s = f->stream;
-  CU_CHECK(cudaMemcpyAsync(f->d_in, in_host, in_bytes, cudaMemcpyHostToDevice, s));
-  rc = mlb_fdtd_process_device(f, f->d_in, f->d_out, n_blocks, s);
-  if (rc != MLB_OK) return rc;
-  CU_CHECK(cudaMemcpyAsync(out_host, f->d_out, out_bytes, cudaMemcpyDeviceToHost, s));
+  MLB_TRY(f->d_in.ensure(in_bytes, "staging"));
+  MLB_TRY(f->d_out.ensure(out_bytes, "staging"));
+  cudaStream_t s = f->stream.get();
+  CU_CHECK(cudaMemcpyAsync(f->d_in.get(), in_host, in_bytes, cudaMemcpyHostToDevice, s));
+  MLB_TRY(mlb_fdtd_process_device(f, f->d_in.get(), f->d_out.get(), n_blocks, s));
+  CU_CHECK(cudaMemcpyAsync(out_host, f->d_out.get(), out_bytes, cudaMemcpyDeviceToHost, s));
   CU_CHECK(cudaStreamSynchronize(s));
   return MLB_OK;
 }
