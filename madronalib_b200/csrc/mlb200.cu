@@ -65,6 +65,16 @@ static int fail(int code, const char* fmt, ...)
     if (rc__ != MLB_OK) return rc__; \
   } while (0)
 
+// The return of a host entry point that has enqueued anything, whatever rc says: wait for every stream the call used,
+// so that no copy still reads or writes the caller's buffers after it returns.  The first error wins.
+static int drain(int rc, std::initializer_list<cudaStream_t> streams)
+{
+  for (cudaStream_t s : streams)
+    if (const cudaError_t e = cudaStreamSynchronize(s); e != cudaSuccess && rc == MLB_OK)
+      rc = fail(MLB_ERR_CUDA, "stream synchronise: %s", cudaGetErrorString(e));
+  return rc;
+}
+
 // ------------------------------------------------------------------------------------------
 // owners of device memory, streams, events and live-handle counts: move-only, failures reported by the explicit
 // alloc / create calls (no exception crosses the C ABI).  A default-constructed owner makes no CUDA runtime call,
@@ -1762,20 +1772,43 @@ static int bus_complete(mlb_graph* g, const MixBusArgs& ba, int n_planes, float*
 {
   mlb_mixbus* b = g->bus;
   if (!b || b->world <= 1 || !b->async) return MLB_OK;
-  static const int dbg = env_int("MLB_BUS_DEBUG", 0);  // timing experiments only: 1 = events but no kernel, 2 = nothing
-  if (dbg == 2) return MLB_OK;
   CU_CHECK(cudaEventRecord(b->ev_posted.get(), stream));
   CU_CHECK(cudaStreamWaitEvent(b->side.get(), b->ev_posted.get(), 0));
-  if (dbg != 1)
-  {
-    mixbus_exchange_kernel<<<(n_planes + kExchangePlanesPerCta - 1) / kExchangePlanesPerCta,
-                             64 * kExchangePlanesPerCta, 0, b->side.get()>>>(mix_dev, ba, n_planes);
-    ++g_launches;
-    CU_CHECK(cudaGetLastError());
-  }
+  mixbus_exchange_kernel<<<(n_planes + kExchangePlanesPerCta - 1) / kExchangePlanesPerCta,
+                           64 * kExchangePlanesPerCta, 0, b->side.get()>>>(mix_dev, ba, n_planes);
+  ++g_launches;
+  CU_CHECK(cudaGetLastError());
   CU_CHECK(cudaEventRecord(b->ev_done[ba.seq % mlb_mixbus::kStage].get(), b->side.get()));
   b->done_pending = true;
   return MLB_OK;
+}
+
+// The mix bus of a call of T blocks whose kernels left their per-group partials in g->partial_cur on `stream`: the
+// reduction into mix_dev and the multi-GPU exchange; with `leave` they run on s_mix, beside the next call's kernel.
+static int mix_tail(mlb_graph* g, float* mix_dev, int T, bool leave, cudaStream_t stream)
+{
+  const int n_groups = (g->V + 31) / 32, n_planes = T * std::max<int>(1, (int)g->outs.size());
+  cudaStream_t ms = leave ? g->s_mix.get() : stream;
+  if (leave)
+  {
+    CU_CHECK(cudaEventRecord(g->ev_main.get(), stream));
+    CU_CHECK(cudaStreamWaitEvent(ms, g->ev_main.get(), 0));
+  }
+  float* scratch = g->partial_cur + (size_t)n_planes * n_groups * MLB_BLOCK;
+  MixBusArgs ba;
+  MLB_TRY(bus_args(g, n_planes, &ba, ms));
+  // (asynchronous mode: 1024-thread CTAs do not fit beside a resident chain CTA and run in the gaps between chain
+  // kernels; 256-thread CTAs that DO run beside it slow the HBM-bound chain kernel down by what they read.  The
+  // reduction costs bandwidth, not latency.)
+  mix_reduce_kernel<<<n_planes, dim3(MLB_BLOCK, 16), 0, ms>>>(g->partial_cur, scratch, mix_dev, n_groups, ba);
+  ++g_launches;
+  CU_CHECK(cudaGetLastError());
+  if (leave)
+  {
+    CU_CHECK(cudaEventRecord(g->ev_mixdone[g->mix_seq & 3u].get(), ms));
+    g->mix_pending = true;
+  }
+  return bus_complete(g, ba, n_planes, mix_dev, ms);
 }
 
 static int env_int(const char* name, int dflt)
@@ -1798,15 +1831,14 @@ static int ensure_partial(mlb_graph* g, int T, int n_groups)
 }
 
 // Launch the fused chain kernel for the voice slice [va, vb) (va a multiple of 32) of the bank.
-// in_dev / out_dev are the FULL planes [T][n][V][64]; the tensor maps, SoA pointers, mix
-// partials and progress words are offset to the slice.
-static int launch_chain_slice(mlb_graph* g, const float* in_dev, float* out_dev, bool want_mix, int T,
+// in_dev / out_dev are the FULL planes [T][in_planes][V][64] / [T][1][V][64]; the tensor maps, SoA
+// pointers, mix partials and progress words are offset to the slice.
+static int launch_chain_slice(mlb_graph* g, const float* in_dev, int in_planes, float* out_dev, bool want_mix, int T,
                               cudaStream_t stream, int va, int vb, int force_chunks = 0)
 {
   const FusedEntry& e = *g->fused;
   const int V = g->V, Vs = vb - va;
   const int groups_total = (V + 31) / 32, n_groups = (Vs + 31) / 32;
-  const int n_in = g->layout.n_inputs;
   int rc;
   ChainArgs a = g->cargs;
   a.state = g->d_state.get() + va;
@@ -1815,7 +1847,7 @@ static int launch_chain_slice(mlb_graph* g, const float* in_dev, float* out_dev,
   a.V = Vs;
   a.T = T;
   a.v_stride = V;
-  a.n_in_planes = std::max(1, n_in);
+  a.n_in_planes = std::max(1, in_planes);
   a.n_out_planes = 1;
   a.out_plane = 0;
   a.n_groups = n_groups;
@@ -1957,25 +1989,91 @@ static int launch_chain_slice(mlb_graph* g, const float* in_dev, float* out_dev,
   return MLB_OK;
 }
 
-extern "C" int mlb_graph_process_device(mlb_graph* g, const float* in_dev, float* out_dev,
-                                        float* mix_dev, int n_blocks, void* stream_v)
+// The checks of a graph call that need no device; the host entry points run them before they enqueue anything.
+static int graph_check(const mlb_graph* g, int n_blocks, int in_planes, const void* in, bool wants_output)
 {
   if (!g) return fail(MLB_ERR_INVALID, "null graph");
   if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive");
-  if (g->layout.n_inputs > 0 && !in_dev) return fail(MLB_ERR_INVALID, "graph has INPUT nodes but in is null");
-  if (g->outs.empty() && (out_dev || mix_dev)) return fail(MLB_ERR_INVALID, "graph has no outputs");
+  if (in_planes > 0 && !in) return fail(MLB_ERR_INVALID, "graph has INPUT nodes but in is null");
+  if (g->outs.empty() && wants_output) return fail(MLB_ERR_INVALID, "graph has no outputs");
   if (g->fdn_node >= 0 && !g->d_ring.get())
     return fail(MLB_ERR_INVALID, "FDN8 graph: call mlb_graph_set_coefs before processing");
-  int rc = ensure_init();
-  if (rc != MLB_OK) return rc;
-  cudaStream_t stream = (cudaStream_t)stream_v;
-  const int V = g->V, T = n_blocks;
-  const int n_groups = (V + 31) / 32;
-  const int n_out = (int)g->outs.size(), n_in = g->layout.n_inputs;
-  if (mix_dev)
+  return MLB_OK;
+}
+
+// The FM3 -> FDN8 kernel; with the mix bus, the per-group partials of its two output planes after it.
+static int launch_fdn(mlb_graph* g, const float* in, int in_planes, float* out, bool want_mix, int T,
+                      cudaStream_t stream)
+{
+  const int V = g->V, n_groups = (V + 31) / 32;
+  // outputs are needed for the mix bus even when the caller does not want them
+  float* planes = out;
+  if (!planes)
   {
-    rc = ensure_partial(g, T, n_groups);
-    if (rc != MLB_OK) return rc;
+    MLB_TRY(g->d_out.ensure((size_t)T * 2 * V * MLB_BLOCK * 4, "staging"));
+    planes = g->d_out.get();
+  }
+  const int rc = launch_fm3_fdn8(g->fargs, g->exact, g->d_state.get(), g->d_coef.get(), g->d_ring.get(), g->d_carry.get(),
+                                 g->ring_len, g->blocks_done, in, planes, V, T, std::max(1, in_planes), stream);
+  if (rc != MLB_OK) return fail(rc, "fdn8 launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+  ++g_launches;
+  if (want_mix)
+  {
+    mix_partial_from_planes_kernel<<<dim3(n_groups, T * 2), MLB_BLOCK, 0, stream>>>(planes, g->partial_cur, V,
+                                                                                    n_groups);
+    ++g_launches;
+  }
+  CU_CHECK(cudaGetLastError());
+  return MLB_OK;
+}
+
+// The graph interpreter kernel.
+static int launch_generic(mlb_graph* g, const float* in, int in_planes, float* out, bool want_mix, int T,
+                          cudaStream_t stream)
+{
+  const int V = g->V, n_groups = (V + 31) / 32;
+  GenericArgs a;
+  memset(&a, 0, sizeof(a));
+  a.nodes = g->d_gnodes.get();
+  a.n_nodes = (int)g->gnodes.size();
+  a.state = g->d_state.get();
+  a.coef = g->d_coef.get();
+  a.in = in;
+  a.out = out;
+  a.mix_partial = want_mix ? g->partial_cur : nullptr;
+  a.V = V, a.T = T, a.n_in = std::max(1, in_planes), a.n_out = std::max<int>(1, (int)g->outs.size());
+  a.n_groups = n_groups, a.n_slots = g->n_slots;
+  a.fdn_ring = g->d_ring.get(), a.fdn_carry = g->d_carry.get(), a.fdn_ring_len = g->ring_len;
+  a.blocks_done = g->blocks_done;
+  a.dmem = g->d_dmem.get();
+  a.scratch_slot = g->scratch_slot;
+  a.stages = g->d_gstages.get();
+  a.n_stages = g->n_stages;
+  a.n_chan = g->n_chan;
+  a.sync = g->d_gsync.get();
+  if (g->n_chan > 0) MLB_TRY(g->d_chan.ensure((size_t)T * g->n_chan * V * MLB_BLOCK * 4, "staging"));
+  a.chan = g->d_chan.get();
+  const int grid = n_groups * g->n_stages;
+  CU_CHECK(cudaMemsetAsync(g->d_gsync.get(), 0, (1 + (size_t)grid) * 4, stream));
+  const size_t smem = (size_t)g->n_slots * kSlotBytes;
+  void (*const fn)(const GenericArgs) = g->exact ? generic_graph_kernel<true> : generic_graph_kernel<false>;
+  CU_CHECK(cudaFuncSetAttribute((const void*)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  fn<<<grid, 32, smem, stream>>>(a);
+  ++g_launches;
+  CU_CHECK(cudaGetLastError());
+  return MLB_OK;
+}
+
+// One call of the graph on device buffers; `in` is [T][in_planes][V][64]: the graph's own plane count from
+// mlb_graph_process_device, the Voice rows (MLB_VOICE_ROWS) from contract E.
+static int graph_process(mlb_graph* g, const float* in, int in_planes, float* out, float* mix, int T,
+                         cudaStream_t stream)
+{
+  MLB_TRY(graph_check(g, T, in_planes, in, out || mix));
+  MLB_TRY(ensure_init());
+  if (mix)
+  {
+    MLB_TRY(ensure_partial(g, T, (g->V + 31) / 32));
     if (g->mix_async)
     {
       // this call's partial buffer; its previous user (two calls ago) must have been reduced
@@ -1987,114 +2085,32 @@ extern "C" int mlb_graph_process_device(mlb_graph* g, const float* in_dev, float
 
   // the timing events are skipped while `stream` is being captured into a CUDA graph
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  cudaStreamIsCapturing(stream, &cap);
+  CU_CHECK(cudaStreamIsCapturing(stream, &cap));
   const bool capturing = (cap != cudaStreamCaptureStatusNone);
-  if (capturing && (g->fdn_node >= 0 || g->has_dmem || (g->bus && g->bus->world > 1) || (g->mix_async && mix_dev)))
+  if (capturing && (g->fdn_node >= 0 || g->has_dmem || (g->bus && g->bus->world > 1) || (g->mix_async && mix)))
     return fail(MLB_ERR_UNSUPPORTED, "CUDA-graph capture of a process call is supported for graphs without delay "
                                      "memory and without a mix bus (their call counters are kernel arguments)");
-  if (!capturing) cudaEventRecord(g->ev0.get(), stream);
+  if (!capturing) CU_CHECK(cudaEventRecord(g->ev0.get(), stream));
   if (g->kind == KIND_FUSED)
-  {
-    rc = launch_chain_slice(g, in_dev, out_dev, mix_dev != nullptr, T, stream, 0, V);
-    if (rc != MLB_OK) return rc;
-  }
+    MLB_TRY(launch_chain_slice(g, in, in_planes, out, mix != nullptr, T, stream, 0, g->V));
   else if (g->kind == KIND_FDN)
-  {
-    // outputs are needed for the mix bus even when the caller does not want them
-    float* planes = out_dev;
-    if (!planes)
-    {
-      MLB_TRY(g->d_out.ensure((size_t)T * 2 * V * MLB_BLOCK * 4, "staging"));
-      planes = g->d_out.get();
-    }
-    rc = launch_fm3_fdn8(g->fargs, g->exact, g->d_state.get(), g->d_coef.get(), g->d_ring.get(), g->d_carry.get(),
-                         g->ring_len, g->blocks_done, in_dev, planes, V, T, std::max(1, n_in), stream);
-    if (rc != MLB_OK) return fail(rc, "fdn8 launch failed: %s", cudaGetErrorString(cudaGetLastError()));
-    ++g_launches;
-    if (mix_dev)
-    {
-      mix_partial_from_planes_kernel<<<dim3(n_groups, T * 2), MLB_BLOCK, 0, stream>>>(planes, g->partial_cur, V,
-                                                                                      n_groups);
-      ++g_launches;
-    }
-  }
+    MLB_TRY(launch_fdn(g, in, in_planes, out, mix != nullptr, T, stream));
   else
-  {
-    GenericArgs a;
-    memset(&a, 0, sizeof(a));
-    a.nodes = g->d_gnodes.get();
-    a.n_nodes = (int)g->gnodes.size();
-    a.state = g->d_state.get();
-    a.coef = g->d_coef.get();
-    a.in = in_dev;
-    a.out = out_dev;
-    a.mix_partial = mix_dev ? g->partial_cur : nullptr;
-    a.V = V, a.T = T, a.n_in = std::max(1, n_in), a.n_out = std::max(1, n_out);
-    a.n_groups = n_groups, a.n_slots = g->n_slots;
-    a.fdn_ring = g->d_ring.get(), a.fdn_carry = g->d_carry.get(), a.fdn_ring_len = g->ring_len;
-    a.blocks_done = g->blocks_done;
-    a.dmem = g->d_dmem.get();
-    a.scratch_slot = g->scratch_slot;
-    a.stages = g->d_gstages.get();
-    a.n_stages = g->n_stages;
-    a.n_chan = g->n_chan;
-    a.sync = g->d_gsync.get();
-    if (g->n_chan > 0) MLB_TRY(g->d_chan.ensure((size_t)T * g->n_chan * V * MLB_BLOCK * 4, "staging"));
-    a.chan = g->d_chan.get();
-    const int grid = n_groups * g->n_stages;
-    CU_CHECK(cudaMemsetAsync(g->d_gsync.get(), 0, (1 + (size_t)grid) * 4, stream));
-    const size_t smem = (size_t)g->n_slots * kSlotBytes;
-    if (g->exact)
-    {
-      CU_CHECK(cudaFuncSetAttribute((const void*)generic_graph_kernel<true>,
-                                    cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      generic_graph_kernel<true><<<grid, 32, smem, stream>>>(a);
-    }
-    else
-    {
-      CU_CHECK(cudaFuncSetAttribute((const void*)generic_graph_kernel<false>,
-                                    cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      generic_graph_kernel<false><<<grid, 32, smem, stream>>>(a);
-    }
-    ++g_launches;
-  }
+    MLB_TRY(launch_generic(g, in, in_planes, out, mix != nullptr, T, stream));
   if (!capturing)
   {
-    cudaEventRecord(g->ev1.get(), stream);
+    CU_CHECK(cudaEventRecord(g->ev1.get(), stream));
     g->timed = true;
   }
-  CU_CHECK(cudaGetLastError());
   if (g->fdn_node >= 0 || g->has_dmem) g->blocks_done += T;
-  if (mix_dev)
-  {
-    // asynchronous mix bus: the reduction leaves the caller's stream here and runs beside the next call's kernel
-    cudaStream_t ms = stream;
-    if (g->mix_async)
-    {
-      CU_CHECK(cudaEventRecord(g->ev_main.get(), stream));
-      CU_CHECK(cudaStreamWaitEvent(g->s_mix.get(), g->ev_main.get(), 0));
-      ms = g->s_mix.get();
-    }
-    float* scratch = g->partial_cur + (size_t)T * std::max(1, n_out) * n_groups * MLB_BLOCK;
-    MixBusArgs ba;
-    rc = bus_args(g, T * std::max(1, n_out), &ba, ms);
-    if (rc != MLB_OK) return rc;
-    // (asynchronous mode: 1024-thread CTAs do not fit beside a resident chain CTA and run in the gaps between chain
-    // kernels; 256-thread CTAs that DO run beside it slow the HBM-bound chain kernel down by what they read.  The
-    // reduction costs bandwidth, not latency.)
-    mix_reduce_kernel<<<T * std::max(1, n_out), dim3(MLB_BLOCK, 16), 0, ms>>>(g->partial_cur, scratch, mix_dev,
-                                                                               n_groups, ba);
-    ++g_launches;
-    CU_CHECK(cudaGetLastError());
-    if (g->mix_async)
-    {
-      CU_CHECK(cudaEventRecord(g->ev_mixdone[g->mix_seq & 3u].get(), ms));
-      g->mix_pending = true;
-    }
-    rc = bus_complete(g, ba, T * std::max(1, n_out), mix_dev, ms);
-    if (rc != MLB_OK) return rc;
-  }
-  return MLB_OK;
+  // asynchronous mix bus (mlb_graph_set_mix_async): the reduction leaves the caller's stream
+  return mix ? mix_tail(g, mix, T, g->mix_async != 0, stream) : MLB_OK;
+}
+
+extern "C" int mlb_graph_process_device(mlb_graph* g, const float* in_dev, float* out_dev,
+                                        float* mix_dev, int n_blocks, void* stream)
+{
+  return graph_process(g, in_dev, g ? g->layout.n_inputs : 0, out_dev, mix_dev, n_blocks, (cudaStream_t)stream);
 }
 
 extern "C" int mlb_graph_set_mix_async(mlb_graph* g, int on)
@@ -2112,102 +2128,107 @@ extern "C" int mlb_graph_set_mix_async(mlb_graph* g, int on)
   return MLB_OK;
 }
 
+// The three-stream pipeline of the host entry points over the pieces [a, b) = [p * per, min(total, (p + 1) * per)) of
+// `total` voices or blocks: piece p goes up on s_h2d (if `up`), runs on the graph's stream once it is there (ev_up[p])
+// and goes down on s_d2h (if `down`) once it has run (ev_k[p]), so that the upload of piece p + 1, the kernels of
+// piece p and the download of piece p - 1 overlap (PCIe is full duplex).  Steps are called as step(a, b, stream).
+// The caller drains the three streams whatever this returns.
+template <class Up, class Run, class Down>
+static int host_pipeline(mlb_graph* g, int total, int per, bool up, bool down, Up upload, Run run, Down download)
+{
+  const int n = (total + per - 1) / per;
+  if (n > mlb_graph::kMaxHostSlices)
+    return fail(MLB_ERR_INVALID, "%d pieces exceed the %d of one host call", n, mlb_graph::kMaxHostSlices);
+  g->last_host_slices = 0;
+  for (int p = 0; p < n; ++p)
+  {
+    const int a = p * per, b = std::min(total, a + per);
+    if (up)
+    {
+      CU_CHECK(upload(a, b, g->s_h2d.get()));
+      CU_CHECK(cudaEventRecord(g->ev_up[p].get(), g->s_h2d.get()));
+      CU_CHECK(cudaStreamWaitEvent(g->stream.get(), g->ev_up[p].get(), 0));
+    }
+    MLB_TRY(run(a, b, g->stream.get()));
+    if (down)
+    {
+      CU_CHECK(cudaEventRecord(g->ev_k[p].get(), g->stream.get()));
+      CU_CHECK(cudaStreamWaitEvent(g->s_d2h.get(), g->ev_k[p].get(), 0));
+      CU_CHECK(download(a, b, g->s_d2h.get()));
+    }
+    g->last_host_slices = p + 1;
+  }
+  return MLB_OK;
+}
+
 extern "C" int mlb_graph_process_host(mlb_graph* g, const float* in_host, float* out_host,
                                       float* mix_host, int n_blocks)
 {
-  if (!g) return fail(MLB_ERR_INVALID, "null graph");
-  if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive");
-  int rc = ensure_init();
-  if (rc != MLB_OK) return rc;
-  const size_t V = (size_t)g->V, T = (size_t)n_blocks;
-  const size_t n_in = (size_t)g->layout.n_inputs, n_out = g->outs.size();
+  const int n_in = g ? g->layout.n_inputs : 0;
+  MLB_TRY(graph_check(g, n_blocks, n_in, in_host, out_host || mix_host));
+  MLB_TRY(ensure_init());
+  const size_t V = (size_t)g->V, T = (size_t)n_blocks, n_out = g->outs.size();
   const size_t in_bytes = T * n_in * V * MLB_BLOCK * 4, out_bytes = T * n_out * V * MLB_BLOCK * 4;
   const size_t mix_bytes = T * n_out * MLB_BLOCK * 4;
-  if (n_in && !in_host) return fail(MLB_ERR_INVALID, "graph has INPUT nodes but in is null");
   if (n_in) MLB_TRY(g->d_in.ensure(in_bytes, "staging"));
   if (out_host) MLB_TRY(g->d_out.ensure(out_bytes, "staging"));
   if (mix_host) MLB_TRY(g->d_mix.ensure(mix_bytes, "staging"));
+  float* d_in = n_in ? g->d_in.get() : nullptr;
+  float* d_out = out_host ? g->d_out.get() : nullptr;
+  float* d_mix = mix_host ? g->d_mix.get() : nullptr;
   cudaStream_t s = g->stream.get();
-  // Large fused banks: pipeline over voice slices so that the H2D copy of slice p+1, the kernel
-  // of slice p and the D2H copy of slice p-1 overlap (three streams; PCIe is full duplex).
-  // A slice is a strided window [T*n][va:vb][64] of the host planes -> cudaMemcpy2DAsync.
-  const int n_slices_env = env_int("MLB_HOST_SLICES", 16);
+  // Large fused banks: pipelined over voice slices (host_pipeline).
+  const int n_slices = std::min(env_int("MLB_HOST_SLICES", 16), (int)mlb_graph::kMaxHostSlices);
   // Only planes that really cross PCIe count: a mix-only call (out_host == NULL) moves 256 B per
   // block and must stay ONE launch -- 16 slice launches of a 4096-voice bank are latency-bound.
   const size_t pcie_bytes = in_bytes + (out_host ? out_bytes : 0);
   const size_t slice_min_bytes = (size_t)env_int("MLB_HOST_SLICE_MIN_MB", 32) << 20;
-  g->last_host_slices = 1;
-  if (g->kind == KIND_FUSED && n_slices_env > 1 && g->V >= 4096 && pcie_bytes >= slice_min_bytes)
+  const bool sliced = g->kind == KIND_FUSED && n_slices > 1 && g->V >= 4096 && pcie_bytes >= slice_min_bytes;
+  // a slice [va, vb) of n planes is the strided window [T * n][va:vb][64] of the planes
+  auto window = [&](float* dst, const float* src, size_t n, int va, int vb, cudaMemcpyKind kind, cudaStream_t st)
   {
-    const int n_slices = std::min(n_slices_env, (int)mlb_graph::kMaxHostSlices);
-    int per = (g->V + n_slices - 1) / n_slices;
-    per = (per + 31) / 32 * 32;
-    const size_t pitch = V * MLB_BLOCK * 4;
-    if (mix_host && (rc = ensure_partial(g, n_blocks, (g->V + 31) / 32)) != MLB_OK) return rc;
-    if (mix_host && (rc = mlb_graph_mix_wait(g, s)) != MLB_OK) return rc;  // an asynchronous reduce may still read the partials
-    int chunks = 0;
-    cudaEventRecord(g->ev0.get(), s);
-    g->last_host_slices = 0;
-    for (int p = 0, va = 0; va < g->V; ++p, va += per)
+    const size_t pitch = V * MLB_BLOCK * 4, at = (size_t)va * MLB_BLOCK;
+    return cudaMemcpy2DAsync(dst + at, pitch, src + at, pitch, (size_t)(vb - va) * MLB_BLOCK * 4, T * n, kind, st);
+  };
+  const int rc = [&]() -> int
+  {
+    if (!sliced)
     {
-      ++g->last_host_slices;
-      const int vb = std::min(g->V, va + per);
-      const size_t width = (size_t)(vb - va) * MLB_BLOCK * 4;
-      if (n_in)
-      {
-        CU_CHECK(cudaMemcpy2DAsync(g->d_in.get() + (size_t)va * MLB_BLOCK, pitch, in_host + (size_t)va * MLB_BLOCK,
-                                   pitch, width, T * n_in, cudaMemcpyHostToDevice, g->s_h2d.get()));
-        CU_CHECK(cudaEventRecord(g->ev_up[p].get(), g->s_h2d.get()));
-        CU_CHECK(cudaStreamWaitEvent(s, g->ev_up[p].get(), 0));
-      }
-      rc = launch_chain_slice(g, n_in ? g->d_in.get() : nullptr, out_host ? g->d_out.get() : nullptr,
-                              mix_host != nullptr, n_blocks, s, va, vb, chunks);
-      if (rc != MLB_OK) return rc;
-      chunks = g->launch_chunks;
-      if (out_host)
-      {
-        CU_CHECK(cudaEventRecord(g->ev_k[p].get(), s));
-        CU_CHECK(cudaStreamWaitEvent(g->s_d2h.get(), g->ev_k[p].get(), 0));
-        CU_CHECK(cudaMemcpy2DAsync(out_host + (size_t)va * MLB_BLOCK, pitch, g->d_out.get() + (size_t)va * MLB_BLOCK,
-                                   pitch, width, T * n_out, cudaMemcpyDeviceToHost, g->s_d2h.get()));
-      }
+      g->last_host_slices = 1;
+      if (n_in) CU_CHECK(cudaMemcpyAsync(d_in, in_host, in_bytes, cudaMemcpyHostToDevice, s));
+      MLB_TRY(graph_process(g, d_in, n_in, d_out, d_mix, n_blocks, s));
+      if (out_host) CU_CHECK(cudaMemcpyAsync(out_host, d_out, out_bytes, cudaMemcpyDeviceToHost, s));
+      if (mix_host) MLB_TRY(mlb_graph_mix_wait(g, s));  // async mix bus: the completion runs on a side stream
+      if (mix_host) CU_CHECK(cudaMemcpyAsync(mix_host, d_mix, mix_bytes, cudaMemcpyDeviceToHost, s));
+      return MLB_OK;
     }
-    cudaEventRecord(g->ev1.get(), s);
+    if (mix_host) MLB_TRY(ensure_partial(g, n_blocks, (g->V + 31) / 32));
+    if (mix_host) MLB_TRY(mlb_graph_mix_wait(g, s));  // an asynchronous reduce may still read the partials
+    CU_CHECK(cudaEventRecord(g->ev0.get(), s));
+    const int per = ((g->V + n_slices - 1) / n_slices + 31) / 32 * 32;
+    MLB_TRY(host_pipeline(
+        g, g->V, per, n_in != 0, out_host != nullptr,
+        [&](int va, int vb, cudaStream_t st) { return window(d_in, in_host, n_in, va, vb, cudaMemcpyHostToDevice, st); },
+        [&](int va, int vb, cudaStream_t st)
+        {
+          // every slice takes the chunk count of the first slice's launch
+          return launch_chain_slice(g, d_in, n_in, d_out, mix_host != nullptr, n_blocks, st, va, vb,
+                                    va ? g->launch_chunks : 0);
+        },
+        [&](int va, int vb, cudaStream_t st) { return window(out_host, d_out, n_out, va, vb, cudaMemcpyDeviceToHost, st); }));
+    CU_CHECK(cudaEventRecord(g->ev1.get(), s));
     g->timed = true;
     if (mix_host)
     {
-      const int n_groups = (g->V + 31) / 32;
-      float* scratch = g->partial_cur + T * std::max<size_t>(1, n_out) * n_groups * MLB_BLOCK;
-      MixBusArgs ba;
-      rc = bus_args(g, (int)(T * std::max<size_t>(1, n_out)), &ba, s);
-      if (rc != MLB_OK) return rc;
-      mix_reduce_kernel<<<(int)(T * std::max<size_t>(1, n_out)), dim3(MLB_BLOCK, 16), 0, s>>>(g->partial_cur, scratch,
-                                                                                            g->d_mix.get(), n_groups, ba);
-      rc = bus_complete(g, ba, (int)(T * std::max<size_t>(1, n_out)), g->d_mix.get(), s);
-      if (rc != MLB_OK) return rc;
-      rc = mlb_graph_mix_wait(g, s);  // the host entry point returns finished results
-      if (rc != MLB_OK) return rc;
-      ++g_launches;
-      CU_CHECK(cudaGetLastError());
-      CU_CHECK(cudaMemcpyAsync(mix_host, g->d_mix.get(), mix_bytes, cudaMemcpyDeviceToHost, s));
+      // the reduction stays on `s`: this call waits for it anyway, and the slices wrote their partials to the first
+      // buffer, whatever the call parity of the asynchronous mix bus
+      MLB_TRY(mix_tail(g, d_mix, n_blocks, false, s));
+      MLB_TRY(mlb_graph_mix_wait(g, s));
+      CU_CHECK(cudaMemcpyAsync(mix_host, d_mix, mix_bytes, cudaMemcpyDeviceToHost, s));
     }
-    CU_CHECK(cudaStreamSynchronize(s));
-    CU_CHECK(cudaStreamSynchronize(g->s_d2h.get()));
     return MLB_OK;
-  }
-  if (n_in) CU_CHECK(cudaMemcpyAsync(g->d_in.get(), in_host, in_bytes, cudaMemcpyHostToDevice, s));
-  rc = mlb_graph_process_device(g, n_in ? g->d_in.get() : nullptr, out_host ? g->d_out.get() : nullptr,
-                                mix_host ? g->d_mix.get() : nullptr, n_blocks, s);
-  if (rc != MLB_OK) return rc;
-  if (out_host) CU_CHECK(cudaMemcpyAsync(out_host, g->d_out.get(), out_bytes, cudaMemcpyDeviceToHost, s));
-  if (mix_host)
-  {
-    rc = mlb_graph_mix_wait(g, s);  // async mix bus: the completion runs on a side stream
-    if (rc != MLB_OK) return rc;
-    CU_CHECK(cudaMemcpyAsync(mix_host, g->d_mix.get(), mix_bytes, cudaMemcpyDeviceToHost, s));
-  }
-  CU_CHECK(cudaStreamSynchronize(s));
-  return MLB_OK;
+  }();
+  return sliced ? drain(rc, {g->s_h2d.get(), s, g->s_d2h.get()}) : drain(rc, {s});
 }
 
 extern "C" int mlb_graph_last_host_slices(const mlb_graph* g) { return g ? g->last_host_slices : -1; }
@@ -2269,7 +2290,8 @@ extern "C" int mlb_map_host(int op, const float* x1, const float* x2, const floa
                             size_t n_rows)
 {
   int nin, nst, nco;
-  if (mlb_op_info(op, &nin, &nst, &nco) != MLB_OK) return fail(MLB_ERR_INVALID, "unknown op %d", op);
+  if (mlb_op_info(op, &nin, &nst, &nco) != MLB_OK || !map_kernel_for(op))
+    return fail(MLB_ERR_INVALID, "op %d is not a stateless elementwise op", op);
   if (n_rows == 0) return MLB_OK;
   if (!x1 || !y || (nin >= 2 && !x2) || (nin >= 3 && !x3)) return fail(MLB_ERR_INVALID, "null operand");
   int rc = ensure_init();
@@ -2293,13 +2315,16 @@ extern "C" int mlb_map_host(int op, const float* x1, const float* x2, const floa
     ++P.allocations;
   }
   const float* h[3] = {x1, x2, x3};
-  for (int k = 0; k < nin && k < 3; ++k)
-    CU_CHECK(cudaMemcpyAsync(P.d[k], h[k], bytes, cudaMemcpyHostToDevice, P.stream));
-  rc = mlb_map_device(op, P.d[0], nin >= 2 ? P.d[1] : nullptr, nin >= 3 ? P.d[2] : nullptr, P.d[3], n_rows, P.stream);
-  if (rc != MLB_OK) return rc;
-  CU_CHECK(cudaMemcpyAsync(y, P.d[3], bytes, cudaMemcpyDeviceToHost, P.stream));
-  CU_CHECK(cudaStreamSynchronize(P.stream));
-  return MLB_OK;
+  rc = [&]() -> int
+  {
+    for (int k = 0; k < nin && k < 3; ++k)
+      CU_CHECK(cudaMemcpyAsync(P.d[k], h[k], bytes, cudaMemcpyHostToDevice, P.stream));
+    MLB_TRY(mlb_map_device(op, P.d[0], nin >= 2 ? P.d[1] : nullptr, nin >= 3 ? P.d[2] : nullptr, P.d[3], n_rows,
+                           P.stream));
+    CU_CHECK(cudaMemcpyAsync(y, P.d[3], bytes, cudaMemcpyDeviceToHost, P.stream));
+    return MLB_OK;
+  }();
+  return drain(rc, {P.stream});
 }
 
 
@@ -2463,21 +2488,23 @@ extern "C" int mlb_voices_process_host(mlb_voices* vb, const mlb_voice_events* e
   MLB_TRY(vb->d_ev.ensure(ev_bytes, "staging"));
   MLB_TRY(vb->d_out.ensure(out_bytes, "staging"));
   cudaStream_t s = vb->stream.get();
-  CU_CHECK(cudaMemcpyAsync(vb->d_ev.get(), events_host, ev_bytes, cudaMemcpyHostToDevice, s));
-  int rc = mlb_voices_process_device(vb, vb->d_ev.get(), vb->d_out.get(), n_blocks, row_mask, s);
-  if (rc != MLB_OK) return rc;
-  const size_t plane = V * MLB_BLOCK * 4;
-  if (row_mask == 0xFFu)
-    CU_CHECK(cudaMemcpyAsync(out_host, vb->d_out.get(), out_bytes, cudaMemcpyDeviceToHost, s));
-  else
-    for (size_t t = 0; t < T; ++t)
-      for (int r = 0; r < MLB_VOICE_ROWS; ++r)
-        if (row_mask & (1u << r))
-          CU_CHECK(cudaMemcpyAsync(reinterpret_cast<char*>(out_host) + (t * MLB_VOICE_ROWS + r) * plane,
-                                   reinterpret_cast<char*>(vb->d_out.get()) + (t * MLB_VOICE_ROWS + r) * plane, plane,
-                                   cudaMemcpyDeviceToHost, s));
-  CU_CHECK(cudaStreamSynchronize(s));
-  return MLB_OK;
+  const int rc = [&]() -> int
+  {
+    CU_CHECK(cudaMemcpyAsync(vb->d_ev.get(), events_host, ev_bytes, cudaMemcpyHostToDevice, s));
+    MLB_TRY(mlb_voices_process_device(vb, vb->d_ev.get(), vb->d_out.get(), n_blocks, row_mask, s));
+    const size_t plane = V * MLB_BLOCK * 4;
+    if (row_mask == 0xFFu)
+      CU_CHECK(cudaMemcpyAsync(out_host, vb->d_out.get(), out_bytes, cudaMemcpyDeviceToHost, s));
+    else
+      for (size_t t = 0; t < T; ++t)
+        for (int r = 0; r < MLB_VOICE_ROWS; ++r)
+          if (row_mask & (1u << r))
+            CU_CHECK(cudaMemcpyAsync(reinterpret_cast<char*>(out_host) + (t * MLB_VOICE_ROWS + r) * plane,
+                                     reinterpret_cast<char*>(vb->d_out.get()) + (t * MLB_VOICE_ROWS + r) * plane,
+                                     plane, cudaMemcpyDeviceToHost, s));
+    return MLB_OK;
+  }();
+  return drain(rc, {s});
 }
 
 
@@ -2485,17 +2512,17 @@ extern "C" int mlb_voices_process_host(mlb_voices* vb, const mlb_voice_events* e
 // the Voice bank writes the rows the graph reads (EventsToSignals::processVector,
 // MLEventsToSignals.cpp:383-470) into a device buffer that IS the graph's input (the bank's out planes
 // have the layout of graph inputs, plane r = row r), and the graph runs on it in the same stream.
-// Pipelined over TIME chunks -- blocks are contiguous in every buffer involved, and both the bank and
-// the graph carry their state from launch to launch -- so that the H2D copy of chunk c+1's records, the
-// two kernels of chunk c and the D2H copy of chunk c-1's output rows overlap.
+// Pipelined over TIME chunks by host_pipeline -- blocks are contiguous in every buffer involved, and both
+// the bank and the graph carry their state from launch to launch -- so that the H2D copy of chunk c+1's
+// records, the kernels of chunk c and the D2H copy of chunk c-1's output rows overlap.
 // mlb_synth_process_buses_host runs the same pipeline with the bus kernel (K10) after the graph.
 
 // The checks both contract-E entry points share; *row_mask = the Voice rows the graph reads.
 static int synth_check(const mlb_voices* vb, const mlb_graph* g, const mlb_voice_events* events_host, int n_blocks,
-                       unsigned* row_mask)
+                       bool wants_output, unsigned* row_mask)
 {
   if (!vb || !g || !events_host) return fail(MLB_ERR_INVALID, "null argument");
-  if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive");
+  MLB_TRY(graph_check(g, n_blocks, MLB_VOICE_ROWS, events_host, wants_output));
   if (vb->V != g->V) return fail(MLB_ERR_INVALID, "voice bank has %d voices, graph has %d", vb->V, g->V);
   *row_mask = 0;
   for (const mlb_node& n : g->nodes)
@@ -2519,90 +2546,45 @@ static int synth_chunk_blocks(const mlb_graph* g, int n_blocks)
   return std::max<int>(Tc, (n_blocks + mlb_graph::kMaxHostSlices - 1) / mlb_graph::kMaxHostSlices);
 }
 
-// The time-chunk loop.  Per chunk [t0, t0 + tc) of Tc blocks: the records go up on g->s_h2d; on the graph's stream
-// the bank writes the rows the graph reads into vb->d_out, and run_chunk(t0, tc, s) launches what reads them; then,
-// if down_host, the chunk's tc * down_per_block floats of down_dev go down on g->s_d2h.  The caller drains the
-// streams (synth_drain) whatever this returns.
-template <class RunChunk>
-static int synth_pipeline(mlb_voices* vb, mlb_graph* g, const mlb_voice_events* events_host, int n_blocks,
-                          unsigned row_mask, int Tc, const float* down_dev, float* down_host, size_t down_per_block,
-                          RunChunk run_chunk)
-{
-  const size_t V = (size_t)g->V, T = (size_t)n_blocks;
-  MLB_TRY(vb->d_ev.ensure(T * V * sizeof(mlb_voice_events), "staging"));
-  MLB_TRY(vb->d_out.ensure((size_t)Tc * MLB_VOICE_ROWS * V * MLB_BLOCK * 4, "staging"));
-  const int saved_inputs = g->layout.n_inputs;
-  g->layout.n_inputs = MLB_VOICE_ROWS;
-  cudaStream_t s = g->stream.get();
-  int rc = MLB_OK, p = 0;
-  for (size_t t0 = 0; t0 < T && rc == MLB_OK; t0 += (size_t)Tc, ++p)
-  {
-    const int tc = (int)std::min<size_t>((size_t)Tc, T - t0);
-    cudaError_t ce = cudaMemcpyAsync(vb->d_ev.get() + t0 * V, events_host + t0 * V,
-                                     (size_t)tc * V * sizeof(mlb_voice_events), cudaMemcpyHostToDevice, g->s_h2d.get());
-    if (ce == cudaSuccess) ce = cudaEventRecord(g->ev_up[p].get(), g->s_h2d.get());
-    if (ce == cudaSuccess) ce = cudaStreamWaitEvent(s, g->ev_up[p].get(), 0);
-    if (ce != cudaSuccess)
-    {
-      rc = fail(MLB_ERR_CUDA, "events H2D: %s", cudaGetErrorString(ce));
-      break;
-    }
-    rc = mlb_voices_process_device(vb, vb->d_ev.get() + t0 * V, vb->d_out.get(), tc, row_mask, s);
-    if (rc != MLB_OK) break;
-    rc = run_chunk(t0, tc, s);
-    if (rc != MLB_OK) break;
-    if (down_host)
-    {
-      ce = cudaEventRecord(g->ev_k[p].get(), s);
-      if (ce == cudaSuccess) ce = cudaStreamWaitEvent(g->s_d2h.get(), g->ev_k[p].get(), 0);
-      if (ce == cudaSuccess)
-        ce = cudaMemcpyAsync(down_host + t0 * down_per_block, down_dev + t0 * down_per_block,
-                             (size_t)tc * down_per_block * 4, cudaMemcpyDeviceToHost, g->s_d2h.get());
-      if (ce != cudaSuccess) rc = fail(MLB_ERR_CUDA, "rows D2H: %s", cudaGetErrorString(ce));
-    }
-  }
-  g->layout.n_inputs = saved_inputs;
-  g->last_host_slices = p;
-  return rc;
-}
-
-// Drain all three streams whatever happened: nothing may still touch the caller's buffers on return.
-static int synth_drain(mlb_graph* g, int rc)
-{
-  cudaStreamSynchronize(g->s_h2d.get());
-  cudaError_t e1 = cudaStreamSynchronize(g->stream.get()), e2 = cudaStreamSynchronize(g->s_d2h.get());
-  if (rc == MLB_OK && (e1 != cudaSuccess || e2 != cudaSuccess))
-    rc = fail(MLB_ERR_CUDA, "synth pipeline: %s", cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
-  return rc;
-}
-
 extern "C" int mlb_synth_process_host(mlb_voices* vb, mlb_graph* g, const mlb_voice_events* events_host,
                                       float* out_host, float* mix_host, int n_blocks)
 {
   unsigned row_mask;
-  int rc = synth_check(vb, g, events_host, n_blocks, &row_mask);
-  if (rc != MLB_OK) return rc;
-  if (g->outs.empty() && (out_host || mix_host)) return fail(MLB_ERR_INVALID, "graph has no outputs");
-  if ((rc = ensure_init()) != MLB_OK) return rc;
+  MLB_TRY(synth_check(vb, g, events_host, n_blocks, out_host || mix_host, &row_mask));
+  MLB_TRY(ensure_init());
   const size_t V = (size_t)g->V, T = (size_t)n_blocks, n_out = g->outs.size();
   const int Tc = synth_chunk_blocks(g, n_blocks);
   if (out_host) MLB_TRY(g->d_out.ensure(T * n_out * V * MLB_BLOCK * 4, "staging"));
   if (mix_host) MLB_TRY(g->d_mix.ensure(T * n_out * MLB_BLOCK * 4, "staging"));
-  rc = synth_pipeline(vb, g, events_host, n_blocks, row_mask, Tc, g->d_out.get(), out_host, n_out * V * MLB_BLOCK,
-                      [&](size_t t0, int tc, cudaStream_t s)
-                      {
-                        float* out = out_host ? g->d_out.get() + t0 * n_out * V * MLB_BLOCK : nullptr;
-                        float* mix = mix_host ? g->d_mix.get() + t0 * n_out * MLB_BLOCK : nullptr;
-                        return mlb_graph_process_device(g, vb->d_out.get(), out, mix, tc, s);
-                      });
-  if (rc == MLB_OK && mix_host)
+  MLB_TRY(vb->d_ev.ensure(T * V * sizeof(mlb_voice_events), "staging"));
+  MLB_TRY(vb->d_out.ensure((size_t)Tc * MLB_VOICE_ROWS * V * MLB_BLOCK * 4, "staging"));
+  const size_t row_floats = n_out * V * MLB_BLOCK;  // output rows per block
+  const int rc = [&]() -> int
   {
-    rc = mlb_graph_mix_wait(g, g->stream.get());
-    if (rc == MLB_OK && cudaMemcpyAsync(mix_host, g->d_mix.get(), T * n_out * MLB_BLOCK * 4, cudaMemcpyDeviceToHost,
-                                        g->stream.get()) != cudaSuccess)
-      rc = fail(MLB_ERR_CUDA, "mix D2H failed");
-  }
-  return synth_drain(g, rc);
+    MLB_TRY(host_pipeline(
+        g, n_blocks, Tc, true, out_host != nullptr,
+        [&](int t0, int t1, cudaStream_t s)
+        {
+          return cudaMemcpyAsync(vb->d_ev.get() + t0 * V, events_host + t0 * V, (t1 - t0) * V * sizeof(mlb_voice_events),
+                                 cudaMemcpyHostToDevice, s);
+        },
+        [&](int t0, int t1, cudaStream_t s) -> int
+        {
+          MLB_TRY(mlb_voices_process_device(vb, vb->d_ev.get() + t0 * V, vb->d_out.get(), t1 - t0, row_mask, s));
+          return graph_process(g, vb->d_out.get(), MLB_VOICE_ROWS, out_host ? g->d_out.get() + t0 * row_floats : nullptr,
+                               mix_host ? g->d_mix.get() + t0 * n_out * MLB_BLOCK : nullptr, t1 - t0, s);
+        },
+        [&](int t0, int t1, cudaStream_t s)
+        {
+          return cudaMemcpyAsync(out_host + t0 * row_floats, g->d_out.get() + t0 * row_floats,
+                                 (t1 - t0) * row_floats * 4, cudaMemcpyDeviceToHost, s);
+        }));
+    if (mix_host) MLB_TRY(mlb_graph_mix_wait(g, g->stream.get()));
+    if (mix_host)
+      CU_CHECK(cudaMemcpyAsync(mix_host, g->d_mix.get(), T * n_out * MLB_BLOCK * 4, cudaMemcpyDeviceToHost, g->stream.get()));
+    return MLB_OK;
+  }();
+  return drain(rc, {g->s_h2d.get(), g->stream.get(), g->s_d2h.get()});
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2672,25 +2654,36 @@ extern "C" int mlb_synth_process_buses_host(mlb_voices* vb, mlb_graph* g, mlb_bu
                                             const mlb_voice_events* events_host, float* bus_host, int n_blocks)
 {
   unsigned row_mask;
-  int rc = synth_check(vb, g, events_host, n_blocks, &row_mask);
-  if (rc != MLB_OK) return rc;
+  MLB_TRY(synth_check(vb, g, events_host, n_blocks, true, &row_mask));
   if (!b || !bus_host) return fail(MLB_ERR_INVALID, "null argument");
   if (b->V != g->V) return fail(MLB_ERR_INVALID, "buses are laid over %d voices, graph has %d", b->V, g->V);
-  if (g->outs.empty()) return fail(MLB_ERR_INVALID, "graph has no outputs");
-  if ((rc = ensure_init()) != MLB_OK) return rc;
+  MLB_TRY(ensure_init());
   const size_t V = (size_t)g->V, T = (size_t)n_blocks, n_out = g->outs.size(), G = (size_t)b->G;
   const int Tc = synth_chunk_blocks(g, n_blocks);
   MLB_TRY(g->d_out.ensure((size_t)Tc * n_out * V * MLB_BLOCK * 4, "staging"));
   MLB_TRY(b->d_out.ensure(T * n_out * G * MLB_BLOCK * 4, "staging"));
-  rc = synth_pipeline(vb, g, events_host, n_blocks, row_mask, Tc, b->d_out.get(), bus_host, n_out * G * MLB_BLOCK,
-                      [&](size_t t0, int tc, cudaStream_t s)
-                      {
-                        int r = mlb_graph_process_device(g, vb->d_out.get(), g->d_out.get(), nullptr, tc, s);
-                        if (r != MLB_OK) return r;
-                        return mlb_buses_sum_device(b, g->d_out.get(), b->d_out.get() + t0 * n_out * G * MLB_BLOCK,
-                                                    (int)n_out, tc, s);
-                      });
-  return synth_drain(g, rc);
+  MLB_TRY(vb->d_ev.ensure(T * V * sizeof(mlb_voice_events), "staging"));
+  MLB_TRY(vb->d_out.ensure((size_t)Tc * MLB_VOICE_ROWS * V * MLB_BLOCK * 4, "staging"));
+  const size_t bus_floats = n_out * G * MLB_BLOCK;  // bus rows per block
+  const int rc = host_pipeline(
+      g, n_blocks, Tc, true, true,
+      [&](int t0, int t1, cudaStream_t s)
+      {
+        return cudaMemcpyAsync(vb->d_ev.get() + t0 * V, events_host + t0 * V, (t1 - t0) * V * sizeof(mlb_voice_events),
+                               cudaMemcpyHostToDevice, s);
+      },
+      [&](int t0, int t1, cudaStream_t s) -> int
+      {
+        MLB_TRY(mlb_voices_process_device(vb, vb->d_ev.get() + t0 * V, vb->d_out.get(), t1 - t0, row_mask, s));
+        MLB_TRY(graph_process(g, vb->d_out.get(), MLB_VOICE_ROWS, g->d_out.get(), nullptr, t1 - t0, s));
+        return mlb_buses_sum_device(b, g->d_out.get(), b->d_out.get() + t0 * bus_floats, (int)n_out, t1 - t0, s);
+      },
+      [&](int t0, int t1, cudaStream_t s)
+      {
+        return cudaMemcpyAsync(bus_host + t0 * bus_floats, b->d_out.get() + t0 * bus_floats, (t1 - t0) * bus_floats * 4,
+                               cudaMemcpyDeviceToHost, s);
+      });
+  return drain(rc, {g->s_h2d.get(), g->stream.get(), g->s_d2h.get()});
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2778,11 +2771,14 @@ extern "C" int mlb_resampler_process_host(mlb_resampler* r, const float* in_host
   MLB_TRY(r->d_in.ensure((size_t)n_blocks_in * row, "staging"));
   MLB_TRY(r->d_out.ensure(std::max<size_t>(1, (size_t)n_out) * row, "staging"));
   cudaStream_t s = r->stream.get();
-  CU_CHECK(cudaMemcpyAsync(r->d_in.get(), in_host, (size_t)n_blocks_in * row, cudaMemcpyHostToDevice, s));
-  MLB_TRY(mlb_resampler_process_device(r, r->d_in.get(), r->d_out.get(), n_blocks_in, n_blocks_out, s));
-  if (n_out > 0) CU_CHECK(cudaMemcpyAsync(out_host, r->d_out.get(), (size_t)n_out * row, cudaMemcpyDeviceToHost, s));
-  CU_CHECK(cudaStreamSynchronize(s));
-  return MLB_OK;
+  const int rc = [&]() -> int
+  {
+    CU_CHECK(cudaMemcpyAsync(r->d_in.get(), in_host, (size_t)n_blocks_in * row, cudaMemcpyHostToDevice, s));
+    MLB_TRY(mlb_resampler_process_device(r, r->d_in.get(), r->d_out.get(), n_blocks_in, n_blocks_out, s));
+    if (n_out > 0) CU_CHECK(cudaMemcpyAsync(out_host, r->d_out.get(), (size_t)n_out * row, cudaMemcpyDeviceToHost, s));
+    return MLB_OK;
+  }();
+  return drain(rc, {s});
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2884,11 +2880,14 @@ extern "C" int mlb_fdtd_process_host(mlb_fdtd* f, const float* in_host, float* o
   MLB_TRY(f->d_in.ensure(in_bytes, "staging"));
   MLB_TRY(f->d_out.ensure(out_bytes, "staging"));
   cudaStream_t s = f->stream.get();
-  CU_CHECK(cudaMemcpyAsync(f->d_in.get(), in_host, in_bytes, cudaMemcpyHostToDevice, s));
-  MLB_TRY(mlb_fdtd_process_device(f, f->d_in.get(), f->d_out.get(), n_blocks, s));
-  CU_CHECK(cudaMemcpyAsync(out_host, f->d_out.get(), out_bytes, cudaMemcpyDeviceToHost, s));
-  CU_CHECK(cudaStreamSynchronize(s));
-  return MLB_OK;
+  const int rc = [&]() -> int
+  {
+    CU_CHECK(cudaMemcpyAsync(f->d_in.get(), in_host, in_bytes, cudaMemcpyHostToDevice, s));
+    MLB_TRY(mlb_fdtd_process_device(f, f->d_in.get(), f->d_out.get(), n_blocks, s));
+    CU_CHECK(cudaMemcpyAsync(out_host, f->d_out.get(), out_bytes, cudaMemcpyDeviceToHost, s));
+    return MLB_OK;
+  }();
+  return drain(rc, {s});
 }
 
 
