@@ -457,6 +457,17 @@ int mlb_router_record_count(const mlb_router* r);
 int mlb_router_unsupported_count(const mlb_router* r);
 void mlb_router_set_mod_cc(mlb_router* r, int cc);   /* EventsToSignals::setModCC (.h:80) */
 int mlb_router_process_vector(mlb_router* r, int start_time, mlb_voice_events* records);
+/* One write of a SmoothedController's inputValue (EventsToSignals::controllers[n], MLEventsToSignals.h:170-180):
+ * a controller event writes controllers[min(source_idx, 128)] (.cpp:743-744, before the CC 120 / 123 cases), and in
+ * the MIDI protocol a channel-pressure event writes controller 128 (.cpp:643-652). */
+typedef struct mlb_controller_change {
+  uint16_t controller;       /* 0..128; larger numbers are read as 128 */
+  uint16_t pad;
+  float value;
+} mlb_controller_change;     /* 8 bytes */
+/* The controller writes of the last mlb_router_process_vector, in the order the reference applies them.  Copies at
+ * most `cap` of them to `out` (which may be NULL when cap is 0) and returns how many there were; -1 on null. */
+int mlb_router_controller_changes(const mlb_router* r, mlb_controller_change* out, int cap);
 
 typedef struct mlb_voices mlb_voices;  /* opaque: V Voice objects on the device */
 
@@ -628,6 +639,53 @@ int mlb_buses_sum_device(mlb_buses* b, const float* rows_dev, float* bus_dev, in
  * buses differ in voice count, the graph has no outputs or reads no Voice row. */
 int mlb_synth_process_buses_host(mlb_voices* vb, mlb_graph* g, mlb_buses* b, const mlb_voice_events* events_host,
                                  float* bus_host, int n_blocks);
+
+/* ---- Smoothed MIDI controllers (K11) -----------------------------------------------------------
+ * Every reference EventsToSignals (one per instrument) owns 129 SmoothedControllers (MLEventsToSignals.h:50,170-180):
+ * per vector each runs output = LinearGlide(inputValue) (MLDSPGens.h:433-515, .cpp:431-435) with a glide of
+ * int(sr * 0.02) samples truncated to whole vectors (.cpp:274-285), and a process function reads the rows through
+ * AudioContext::getInputController(n).  A controller bank holds G instruments x C requested controllers (numbers
+ * 0..128, any order, no repeats): only these are stored and produced; writes to the others are ignored.
+ * Input per block t: the changes of instrument g are changes[offsets[t][g] .. offsets[t][g + 1]) (offsets
+ * [T][G + 1] int32, indexes into `changes`), in event order: the last write to a controller in a block wins, and
+ * an inputValue persists across blocks.  The rows are the reference's bit for bit, -0, +-inf, NaN and subnormals
+ * included.  Output [T][n_planes][N][64]: controller k of the list goes to plane plane0 + k; N = G (instrument rows)
+ * or, after mlb_controllers_set_voice_map, N = V, every voice getting its instrument's row (+0 for a voice of no
+ * instrument): the layout of a voice graph's INPUT planes. */
+typedef struct mlb_controllers mlb_controllers;
+/* protocol: 0 MIDI, 1 MPE (mlb_router_create's); it must match the voice bank's MLB_VOICES_MIDI flag in
+ * mlb_synth_process_controllers_host.  Arguments are validated on the host; MLB_ERR_INVALID names the offending
+ * controller.  A live bank counts toward mlb_init's one-device rule. */
+int mlb_controllers_create(int n_instruments, float sample_rate, int protocol, const int32_t* controllers,
+                           int n_controllers, mlb_controllers** out);
+int mlb_controllers_destroy(mlb_controllers* cb);
+int mlb_controllers_clear(mlb_controllers* cb);   /* every controller back to inputValue = target = 0, idle */
+/* state words [4][C][G] uint32: inputValue, LinearGlide::mTargetValue, mVectorsRemaining (int32), step (the float
+ * bits of mStepVec); rows [C][G][64] = LinearGlide::mCurrVec.  get_state returns an idle glide's (remaining < 0)
+ * row as its target, and set_state reads only the rows of moving glides: an idle row always equals its target. */
+int mlb_controllers_get_state(mlb_controllers* cb, uint32_t* words, float* rows);
+int mlb_controllers_set_state(mlb_controllers* cb, const uint32_t* words, const float* rows);
+/* voice_instrument[V]: the instrument of each voice, or -1; NULL goes back to instrument rows */
+int mlb_controllers_set_voice_map(mlb_controllers* cb, const int32_t* voice_instrument, int n_voices);
+/* one launch for n_blocks vectors, no allocation, no synchronisation (capturable into a CUDA graph) */
+int mlb_controllers_process_device(mlb_controllers* cb, const int32_t* offsets_dev,
+                                   const mlb_controller_change* changes_dev, float* out_dev, int plane0, int n_planes,
+                                   int n_blocks, void* stream);
+/* host buffers: offsets are checked (non-decreasing per block, within [0, n_changes]) before anything is copied */
+int mlb_controllers_process_host(mlb_controllers* cb, const int32_t* offsets_host,
+                                 const mlb_controller_change* changes_host, int n_changes, float* out_host,
+                                 int plane0, int n_planes, int n_blocks);
+/* Contract E with controller planes (AudioContext::getInputController(n) -> graph INPUT planes): the graph's input
+ * per block is the 8 Voice rows, then the C controller rows in the bank's list order (INPUT plane 8 + k is
+ * controller k of the list).  events_host [T][V] as for mlb_synth_process_host; ctrl_offsets_host [T][G + 1] into
+ * ctrl_changes_host, checked before anything is copied; out_host [T][n_out][V][64] or NULL; mix_host [T][n_out][64]
+ * or NULL.  The pipeline of mlb_synth_process_host; returns when its copies are finished, also on failure.
+ * MLB_ERR_INVALID when the bank, the controller bank's voice map (mlb_controllers_set_voice_map) and the graph differ
+ * in voice count, the protocols differ (MPE bank vs MLB_VOICES_MIDI), or the graph reads a plane beyond 8 + C - 1. */
+int mlb_synth_process_controllers_host(mlb_voices* vb, mlb_controllers* cb, mlb_graph* g,
+                                       const mlb_voice_events* events_host, const int32_t* ctrl_offsets_host,
+                                       const mlb_controller_change* ctrl_changes_host, float* out_host,
+                                       float* mix_host, int n_blocks);
 
 #ifdef __cplusplus
 }

@@ -718,6 +718,48 @@ inline void processEventsToBuses(VoiceBank& voices, DeviceBank& bank, Buses& bus
   check(mlb_synth_process_buses_host(voices.handle(), bank.handle(), buses.handle(), events, bus, nBlocks));
 }
 
+// ---- ControllerBank: the smoothed MIDI controllers of G instruments (mlb_controllers_*), what
+// AudioContext::getInputController(n) returns, for the requested controller numbers only ----
+class ControllerBank
+{
+  mlb_controllers* c_ = nullptr;
+  int instruments_ = 0, controllers_ = 0;
+
+ public:
+  // protocol 0 MIDI, 1 MPE; controllers: numbers 0..128, no repeats
+  ControllerBank(int nInstruments, float sampleRate, int protocol, const int32_t* controllers, int nControllers)
+      : instruments_(nInstruments), controllers_(nControllers)
+  {
+    check(mlb_controllers_create(nInstruments, sampleRate, protocol, controllers, nControllers, &c_));
+  }
+  ~ControllerBank() { mlb_controllers_destroy(c_); }
+  ControllerBank(const ControllerBank&) = delete;
+  ControllerBank& operator=(const ControllerBank&) = delete;
+  int instruments() const { return instruments_; }
+  int controllers() const { return controllers_; }
+  mlb_controllers* handle() const { return c_; }
+  void clear() { check(mlb_controllers_clear(c_)); }
+  // voiceInstrument[nVoices]: each voice's instrument or -1; nullptr goes back to instrument rows
+  void setVoiceMap(const int32_t* voiceInstrument, int nVoices) { check(mlb_controllers_set_voice_map(c_, voiceInstrument, nVoices)); }
+  // device buffers, asynchronous on `stream`: offsets [nBlocks][instruments + 1] into changes ->
+  // out [nBlocks][nPlanes][instruments or voices][64], controller k in plane plane0 + k
+  void processDevice(const int32_t* offsets, const mlb_controller_change* changes, float* out, int plane0, int nPlanes,
+                     int nBlocks, void* stream = nullptr)
+  {
+    check(mlb_controllers_process_device(c_, offsets, changes, out, plane0, nPlanes, nBlocks, stream));
+  }
+};
+
+// processEvents with controller planes (mlb_synth_process_controllers_host): the graph's INPUT planes are the 8 Voice
+// rows, then the controllers' rows in list order; records and change lists in, the graph's rows / mix out.
+inline void processEventsWithControllers(VoiceBank& voices, ControllerBank& controllers, DeviceBank& bank,
+                                         const mlb_voice_events* events, const int32_t* offsets,
+                                         const mlb_controller_change* changes, float* out, float* mix, int nBlocks)
+{
+  check(mlb_synth_process_controllers_host(voices.handle(), controllers.handle(), bank.handle(), events, offsets,
+                                           changes, out, mix, nBlocks));
+}
+
 // ---- Resampler: Upsampler(octaves) / Downsampler(octaves) x V on the GPU (mlb_resampler_*) ----
 class Resampler
 {

@@ -84,6 +84,9 @@ class VoiceRouter
   bool awake() const { return awake_; }
   int newestVoice() const { return newestVoice_ - 1; }
   int unsupportedEvents() const { return unsupported_; }
+  // the writes of SmoothedController inputValues of the last processVector, in the order they were applied:
+  // controller events and, in the MIDI protocol, channel pressure (controller 128)
+  const std::vector<mlb_controller_change>& controllerChanges() const { return changes_; }
 
   // addEvent, .cpp:352-368: insert sorted by (time, type)
   void addEvent(const Event& e)
@@ -98,9 +101,11 @@ class VoiceRouter
   // processVector, .cpp:372-418: route the events in [startTime, startTime + 64) and write one record
   // per voice (records[i] belongs to voice i + 1 of the reference, i < polyphony).  Returns the number
   // of note events that did not fit into a record (MLB_VOICE_MAX_EVENTS per voice and vector).
+  // The vector's controller writes are collected on the side (controllerChanges()).
   int processVector(int startTime, mlb_voice_events* records)
   {
     overflow_ = 0;
+    changes_.clear();
     records_ = records;
     for (int i = 0; i < recordCount(); ++i) std::memset(&records[i], 0, sizeof(mlb_voice_events));
     const int endTime = startTime + MLB_BLOCK;
@@ -178,6 +183,14 @@ class VoiceRouter
     }
   }
 
+  void addChange(int ctrl, float val)
+  {
+    mlb_controller_change c{};
+    c.controller = (uint16_t)ctrl;
+    c.value = val;
+    changes_.push_back(c);
+  }
+
   int countHeldNotes() const  // .cpp:463-474
   {
     int n = 0;
@@ -234,7 +247,10 @@ class VoiceRouter
         break;
       case kChannelPressure:  // .cpp:634-670
         if (protocol_ == kMIDI)  // controllers[128].inputValue, one smoother copy per voice
+        {
+          addChange(kChannelPressureControllerIdx, e.value1);
           for (int v = 1; v < polyphony_ + 1; ++v) setCurrent(v, MLB_SET_PRESSURE, e.value1);
+        }
         else if (e.channel == 1)
           setCurrent(0, MLB_SET_Z, e.value1);
         else if (e.channel != 0)
@@ -303,6 +319,7 @@ class VoiceRouter
   {
     const float val = e.value1;
     const int ctrl = std::min<int>(e.sourceIdx, kChannelPressureControllerIdx);
+    addChange(ctrl, val);  // controllers[ctrl].inputValue = val, before the special cases
     if (ctrl == kChannelPressureControllerIdx && protocol_ == kMIDI)  // controllers[ctrl].inputValue = val
       for (int v = 1; v < polyphony_ + 1; ++v) setCurrent(v, MLB_SET_PRESSURE, val);
     if (ctrl == 120)
@@ -345,6 +362,7 @@ class VoiceRouter
   std::array<VoiceMirror, kMaxVoices + 1> voices_{};
   std::array<KeyState, kMaxPhysicalKeys> keyStates_{};
   std::vector<Event> events_;
+  std::vector<mlb_controller_change> changes_;
   mlb_voice_events* records_{nullptr};
   Protocol protocol_{kMIDI};
   int polyphony_{0};

@@ -85,6 +85,16 @@ def lib() -> ctypes.CDLL:
     L.mlb_router_set_mod_cc.argtypes = [_vp, ctypes.c_int]
     L.mlb_router_set_mod_cc.restype = None
     L.mlb_router_process_vector.argtypes = [_vp, ctypes.c_int, _vp]
+    L.mlb_router_controller_changes.argtypes = [_vp, _vp, ctypes.c_int]
+    L.mlb_controllers_create.argtypes = [ctypes.c_int, _cf, ctypes.c_int, _vp, ctypes.c_int, _vp]
+    L.mlb_controllers_destroy.argtypes = [_vp]
+    L.mlb_controllers_clear.argtypes = [_vp]
+    L.mlb_controllers_get_state.argtypes = [_vp, _vp, _vp]
+    L.mlb_controllers_set_state.argtypes = [_vp, _vp, _vp]
+    L.mlb_controllers_set_voice_map.argtypes = [_vp, _vp, ctypes.c_int]
+    L.mlb_controllers_process_device.argtypes = [_vp, _vp, _vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
+    L.mlb_controllers_process_host.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp, ctypes.c_int, ctypes.c_int,
+                                               ctypes.c_int]
     L.mlb_resampler_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
     L.mlb_resampler_destroy.argtypes = [_vp]
     L.mlb_resampler_clear.argtypes = [_vp]
@@ -108,6 +118,7 @@ def lib() -> ctypes.CDLL:
     L.mlb_buses_destroy.argtypes = [_vp]
     L.mlb_buses_sum_device.argtypes = [_vp, _vp, _vp, ctypes.c_int, ctypes.c_int, _vp]
     L.mlb_synth_process_buses_host.argtypes = [_vp, _vp, _vp, _vp, _vp, ctypes.c_int]
+    L.mlb_synth_process_controllers_host.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int]
     L.mlb_graph_process_host.argtypes = [_vp, _vp, _vp, _vp, ctypes.c_int]
     L.mlb_graph_last_kernel_ms.argtypes = [_vp, _vp]
     L.mlb_graph_last_host_slices.argtypes = [_vp]
@@ -180,7 +191,8 @@ def kernel_launches() -> int:
 
 
 def live_handles() -> int:
-    """Graphs, voice banks, bus layouts, resamplers, FDTD banks and mix buses alive in this process."""
+    """Graphs, voice banks, bus layouts, controller banks, resamplers, FDTD banks and mix buses alive in this
+    process."""
     return int(lib().mlb_live_handles())
 
 
@@ -396,6 +408,31 @@ class VoiceGraph(_Handle):
                                             _ptr(mix) if want_mix else None, T))
         return out, mix
 
+    def process_events_controllers_host(self, bank: "VoiceBank", controllers: "ControllerBank", events: np.ndarray,
+                                        offsets: np.ndarray, changes: np.ndarray, want_out: bool = True,
+                                        want_mix: bool = False):
+        """Contract E with controller planes (mlb_synth_process_controllers_host): event records [T][V] and a controller
+        change list (offsets [T][G + 1], changes) in, the graph's rows / mix bus out.  INPUT planes 0..7 are the
+        Voice rows of ``bank``, plane 8 + k controller k of ``controllers`` (which needs a voice map of this graph's
+        voices); nothing but records and changes crosses PCIe on the way in."""
+        s, V = self.spec, self.n_voices
+        if not (isinstance(events, np.ndarray) and events.ndim == 2 and events.shape[1] == V and
+                events.dtype.itemsize == 72 and events.flags["C_CONTIGUOUS"]):
+            raise ValueError("process_events_controllers_host: `events` must be a C-contiguous [T][V] array of 72-byte "
+                             "records")
+        T = int(events.shape[0])
+        off = np.ascontiguousarray(offsets, np.int32)
+        if off.shape != (T, controllers.n_instruments + 1):
+            raise ValueError(f"process_events_controllers_host: offsets must be [{T}][{controllers.n_instruments + 1}], "
+                             f"got {off.shape}")
+        ch = np.ascontiguousarray(changes, CONTROLLER_CHANGE_DTYPE)
+        out = np.empty((T, s.n_out, V, BLOCK), np.float32) if want_out else None
+        mix = np.empty((T, s.n_out, BLOCK), np.float32) if want_mix else None
+        _check(lib().mlb_synth_process_controllers_host(bank._h, controllers._h, self._h, events.ctypes.data,
+                                                        off.ctypes.data, ch.ctypes.data if ch.size else None,
+                                                        _ptr(out), _ptr(mix), T))
+        return out, mix
+
     def process_events_buses_host(self, bank: "VoiceBank", buses: "Buses", events: np.ndarray,
                                   out: Optional[np.ndarray] = None) -> np.ndarray:
         """Contract E with per-instrument output (mlb_synth_process_buses_host): event records [T][V] in, the bus rows
@@ -548,6 +585,92 @@ class Buses(_Handle):
                                           stream or None))
 
 
+CONTROLLER_CHANGE_DTYPE = np.dtype([("controller", "<u2"), ("pad", "<u2"), ("value", "<f4")])  # mlb_controller_change
+
+
+class ControllerBank(_Handle):
+    """G instruments x C requested MIDI controllers (mlb_controllers_*): the SmoothedControllers of one reference
+    EventsToSignals per instrument (MLEventsToSignals.h:170-180), i.e. what AudioContext::getInputController(n)
+    returns, bit for bit.  Input per block: a CSR change list, offsets [T][G + 1] into changes
+    (CONTROLLER_CHANGE_DTYPE), each instrument's writes in event order; output [T][n_planes][N][64] with controller
+    k of the list in plane plane0 + k and N = G, or N = V after set_voice_map (every voice gets its instrument's row,
+    a voice of instrument -1 gets +0)."""
+
+    _destroy = "mlb_controllers_destroy"
+
+    MIDI, MPE = 0, 1
+    N_WORDS = 4  # state words: inputValue, target, vectorsRemaining, step
+
+    def __init__(self, n_instruments: int, controllers, sample_rate: float = 48000.0, protocol: int = 0):
+        ctrl = np.ascontiguousarray(controllers, np.int32)
+        if ctrl.ndim != 1:
+            raise ValueError(f"ControllerBank: `controllers` must be a 1-D list of numbers, got shape {ctrl.shape}")
+        self.n_instruments, self.controllers = int(n_instruments), [int(c) for c in ctrl]
+        self.n_controllers, self.protocol, self.n_voices = len(self.controllers), int(protocol), 0
+        h = ctypes.c_void_p()
+        _check(lib().mlb_controllers_create(self.n_instruments, sample_rate, self.protocol, ctrl.ctypes.data,
+                                            self.n_controllers, ctypes.byref(h)))
+        self._h = h
+
+    def clear(self) -> None:
+        _check(lib().mlb_controllers_clear(self._h))
+
+    def get_state(self):
+        """(words [4][C][G] uint32, rows [C][G][64] f32); an idle glide's row is its target."""
+        C, G = self.n_controllers, self.n_instruments
+        words = np.zeros((self.N_WORDS, C, G), np.uint32)
+        rows = np.zeros((C, G, BLOCK), np.float32)
+        _check(lib().mlb_controllers_get_state(self._h, words.ctypes.data, rows.ctypes.data))
+        return words, rows
+
+    def set_state(self, words: np.ndarray, rows: np.ndarray) -> None:
+        C, G = self.n_controllers, self.n_instruments
+        w = np.ascontiguousarray(words, np.uint32)
+        r = np.ascontiguousarray(rows, np.float32)
+        if w.shape != (self.N_WORDS, C, G) or r.shape != (C, G, BLOCK):
+            raise ValueError(f"set_state: words must be [4][{C}][{G}] and rows [{C}][{G}][64], got {w.shape} and "
+                             f"{r.shape}")
+        _check(lib().mlb_controllers_set_state(self._h, w.ctypes.data, r.ctypes.data))
+
+    def set_voice_map(self, voice_instrument) -> None:
+        """voice_instrument[V]: each voice's instrument or -1; None goes back to instrument rows."""
+        if voice_instrument is None:
+            _check(lib().mlb_controllers_set_voice_map(self._h, None, 0))
+            self.n_voices = 0
+            return
+        vm = np.ascontiguousarray(voice_instrument, np.int32)
+        _check(lib().mlb_controllers_set_voice_map(self._h, vm.ctypes.data, int(vm.shape[0])))
+        self.n_voices = int(vm.shape[0])
+
+    def process_host(self, offsets: np.ndarray, changes: np.ndarray, out: Optional[np.ndarray] = None,
+                     plane0: int = 0, n_planes: Optional[int] = None) -> np.ndarray:
+        """offsets [T][G + 1] int32, changes (CONTROLLER_CHANGE_DTYPE) -> out [T][n_planes][N][64]; planes outside
+        [plane0, plane0 + C) of a given `out` are left as they are."""
+        off = np.ascontiguousarray(offsets, np.int32)
+        if off.ndim != 2 or off.shape[1] != self.n_instruments + 1:
+            raise ValueError(f"process_host: offsets must be [T][{self.n_instruments + 1}], got {off.shape}")
+        ch = np.ascontiguousarray(changes, CONTROLLER_CHANGE_DTYPE)
+        T = int(off.shape[0])
+        P = self.n_controllers if n_planes is None else int(n_planes)
+        shape = (T, P, self.n_voices or self.n_instruments, BLOCK)
+        if out is None:
+            out = np.zeros(shape, np.float32)
+        if not (isinstance(out, np.ndarray) and out.dtype == np.float32 and out.flags["C_CONTIGUOUS"] and
+                out.shape == shape):
+            raise ValueError(f"process_host: `out` must be a C-contiguous float32 array of shape {shape}")
+        _check(lib().mlb_controllers_process_host(self._h, off.ctypes.data, ch.ctypes.data if ch.size else None,
+                                                  int(ch.size), out.ctypes.data, int(plane0), P, T))
+        return out
+
+    def process_device(self, offsets, changes, out, n_blocks: int, plane0: int = 0, n_planes: Optional[int] = None,
+                       stream: int = 0) -> None:
+        """Device buffers (torch tensors / ints); asynchronous on ``stream``, one kernel launch, no allocation or
+        synchronisation (capturable into a CUDA graph)."""
+        P = self.n_controllers if n_planes is None else int(n_planes)
+        _check(lib().mlb_controllers_process_device(self._h, _ptr(offsets), _ptr(changes), _ptr(out), int(plane0), P,
+                                                    int(n_blocks), stream or None))
+
+
 class ResamplerBank(_Handle):
     """Upsampler(octaves) / Downsampler(octaves) x V (SURVEY 8f row 4).  direction: 0 up, 1 down."""
 
@@ -661,3 +784,12 @@ class EventRouter(_Handle):
         """records: array of n_records elements of workloads.VOICE_EVENTS_DTYPE (written in place)."""
         assert records.dtype.itemsize == 72 and records.size == self.n_records and records.flags["C_CONTIGUOUS"]
         return int(lib().mlb_router_process_vector(self._h, start_time, records.ctypes.data))
+
+    def controller_changes(self) -> np.ndarray:
+        """The controller writes of the last process_vector, in the order they were applied (CONTROLLER_CHANGE_DTYPE):
+        controller events (numbers above 128 read as 128) and, in MIDI mode, channel pressure as controller 128."""
+        n = int(lib().mlb_router_controller_changes(self._h, None, 0))
+        out = np.zeros(n, CONTROLLER_CHANGE_DTYPE)
+        if n:
+            lib().mlb_router_controller_changes(self._h, out.ctypes.data, n)
+        return out

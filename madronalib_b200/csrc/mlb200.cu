@@ -29,6 +29,7 @@
 #include "resample_kernel.cuh"
 #include "fdtd_kernel.cuh"
 #include "bus_kernel.cuh"
+#include "controller_kernel.cuh"
 #include "generic_kernel.cuh"
 
 using namespace mlb;
@@ -2429,14 +2430,17 @@ extern "C" int mlb_voices_set_main_voices(mlb_voices* vb, const int32_t* main_vo
   return MLB_OK;
 }
 
-extern "C" int mlb_voices_process_device(mlb_voices* vb, const mlb_voice_events* events_dev, float* out_dev,
-                                         int n_blocks, unsigned row_mask, void* stream)
+// out_dev [T][out_planes][V][64]: the Voice rows in planes 0..7 of each block (contract E with controller planes
+// leaves room for the controller rows after them)
+static int voices_launch(mlb_voices* vb, const mlb_voice_events* events_dev, float* out_dev, int n_blocks,
+                         unsigned row_mask, int out_planes, void* stream)
 {
   if (!vb || !events_dev || (!out_dev && (row_mask & 0xFFu))) return fail(MLB_ERR_INVALID, "null argument");
   if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive");
   VoiceArgs a;
   a.ev = events_dev;
   a.out = out_dev;
+  a.out_block = (size_t)out_planes * vb->V * MLB_BLOCK;
   a.state = vb->d_state.get();
   a.coef = vb->d_coef.get();
   a.grows = vb->d_grows.get();
@@ -2469,11 +2473,18 @@ extern "C" int mlb_voices_process_device(mlb_voices* vb, const mlb_voice_events*
   {
     const size_t n4 = (size_t)n_blocks * vb->V * 16;
     const int grid = (int)std::min<size_t>((n4 + 255) / 256, (size_t)g_sm_count * 16);
-    voice_mpe_add_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(out_dev, vb->d_main.get(), vb->V, n_blocks, a.row_mask);
+    voice_mpe_add_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(out_dev, vb->d_main.get(), vb->V, n_blocks, a.row_mask,
+                                                                  out_planes);
     ++g_launches;
     CU_CHECK(cudaGetLastError());
   }
   return MLB_OK;
+}
+
+extern "C" int mlb_voices_process_device(mlb_voices* vb, const mlb_voice_events* events_dev, float* out_dev,
+                                         int n_blocks, unsigned row_mask, void* stream)
+{
+  return voices_launch(vb, events_dev, out_dev, n_blocks, row_mask, MLB_VOICE_ROWS, stream);
 }
 
 extern "C" int mlb_voices_process_host(mlb_voices* vb, const mlb_voice_events* events_host, float* out_host,
@@ -2518,30 +2529,36 @@ extern "C" int mlb_voices_process_host(mlb_voices* vb, const mlb_voice_events* e
 // mlb_synth_process_buses_host runs the same pipeline with the bus kernel (K10) after the graph.
 
 // The checks both contract-E entry points share; *row_mask = the Voice rows the graph reads.
+// n_planes: the input planes per block, the 8 Voice rows and any controller planes after them.
 static int synth_check(const mlb_voices* vb, const mlb_graph* g, const mlb_voice_events* events_host, int n_blocks,
-                       bool wants_output, unsigned* row_mask)
+                       bool wants_output, unsigned* row_mask, int n_planes = MLB_VOICE_ROWS)
 {
   if (!vb || !g || !events_host) return fail(MLB_ERR_INVALID, "null argument");
-  MLB_TRY(graph_check(g, n_blocks, MLB_VOICE_ROWS, events_host, wants_output));
+  MLB_TRY(graph_check(g, n_blocks, n_planes, events_host, wants_output));
   if (vb->V != g->V) return fail(MLB_ERR_INVALID, "voice bank has %d voices, graph has %d", vb->V, g->V);
   *row_mask = 0;
+  bool reads = false;
   for (const mlb_node& n : g->nodes)
     if (n.op == MLB_OP_INPUT)
     {
-      if (n.iarg < 0 || n.iarg >= MLB_VOICE_ROWS)
-        return fail(MLB_ERR_INVALID, "graph INPUT plane %d is not a Voice row (0..%d)", n.iarg, MLB_VOICE_ROWS - 1);
-      *row_mask |= 1u << n.iarg;
+      if (n.iarg < 0 || n.iarg >= n_planes)
+        return n_planes == MLB_VOICE_ROWS
+                   ? fail(MLB_ERR_INVALID, "graph INPUT plane %d is not a Voice row (0..%d)", n.iarg, MLB_VOICE_ROWS - 1)
+                   : fail(MLB_ERR_INVALID, "graph INPUT plane %d is not a Voice row or controller plane (0..%d)", n.iarg,
+                          n_planes - 1);
+      if (n.iarg < MLB_VOICE_ROWS) *row_mask |= 1u << n.iarg;
+      reads = true;
     }
-  if (!*row_mask) return fail(MLB_ERR_INVALID, "graph reads no Voice row (no INPUT node)");
+  if (!reads) return fail(MLB_ERR_INVALID, "graph reads no Voice row (no INPUT node)");
   return MLB_OK;
 }
 
 // Blocks per time chunk: rows of one chunk stay under ~1 GB (8 planes per block are addressed, only the masked
 // ones are touched), and a call has at most kMaxHostSlices chunks.
-static int synth_chunk_blocks(const mlb_graph* g, int n_blocks)
+static int synth_chunk_blocks(const mlb_graph* g, int n_blocks, int n_planes = MLB_VOICE_ROWS)
 {
   int Tc = env_int("MLB_SYNTH_CHUNK_BLOCKS", 0);
-  if (Tc <= 0) Tc = (int)std::max<size_t>(1, ((size_t)1 << 30) / (MLB_VOICE_ROWS * (size_t)g->V * MLB_BLOCK * 4));
+  if (Tc <= 0) Tc = (int)std::max<size_t>(1, ((size_t)1 << 30) / (n_planes * (size_t)g->V * MLB_BLOCK * 4));
   Tc = std::min<int>(Tc, n_blocks);
   return std::max<int>(Tc, (n_blocks + mlb_graph::kMaxHostSlices - 1) / mlb_graph::kMaxHostSlices);
 }
@@ -2683,6 +2700,286 @@ extern "C" int mlb_synth_process_buses_host(mlb_voices* vb, mlb_graph* g, mlb_bu
         return cudaMemcpyAsync(bus_host + t0 * bus_floats, b->d_out.get() + t0 * bus_floats, (t1 - t0) * bus_floats * 4,
                                cudaMemcpyDeviceToHost, s);
       });
+  return drain(rc, {g->s_h2d.get(), g->stream.get(), g->s_d2h.get()});
+}
+
+// ------------------------------------------------------------------------------------------
+// Smoothed MIDI controllers (K11, controller_kernel.cuh)
+
+struct mlb_controllers
+{
+  // declared first, so released last: the buffers below are freed first, and cudaFree waits for the device
+  LiveCount live;
+  Stream stream;
+  int G = 0, C = 0, protocol = 0;
+  int V = 0;  // voices of the voice map; 0: instrument rows
+  float per_f = 0.f, dy = 0.f;
+  DevBuf<int32_t> d_ctrl;   // [C] controller numbers
+  DevBuf<uint32_t> d_state; // [CS_COUNT][C][G]
+  DevBuf<float> d_rows;     // [C][G][64]
+  DevBuf<int32_t> d_vmap;   // [G + 2] offsets, then [V] voices grouped by instrument, the unmapped ones last
+  DevBuf<int32_t> d_off;    // staging of the host entry points
+  DevBuf<mlb_controller_change> d_ch;
+  DevBuf<float> d_out;
+};
+
+extern "C" int mlb_controllers_destroy(mlb_controllers* cb)
+{
+  delete cb;
+  return MLB_OK;
+}
+
+extern "C" int mlb_controllers_clear(mlb_controllers* cb)
+{
+  if (!cb) return fail(MLB_ERR_INVALID, "null controller bank");
+  const size_t CG = (size_t)cb->C * cb->G;
+  std::vector<uint32_t> st((size_t)CS_COUNT * CG, 0u);
+  std::fill_n(st.begin() + CS_REM * CG, CG, 0xFFFFFFFFu);  // LinearGlide::mVectorsRemaining{-1}
+  CU_CHECK(cudaMemcpy(cb->d_state.get(), st.data(), st.size() * 4, cudaMemcpyHostToDevice));
+  CU_CHECK(cudaMemset(cb->d_rows.get(), 0, cb->d_rows.bytes()));
+  return MLB_OK;
+}
+
+extern "C" int mlb_controllers_create(int n_instruments, float sample_rate, int protocol, const int32_t* controllers,
+                                      int n_controllers, mlb_controllers** out)
+{
+  if (!out) return fail(MLB_ERR_INVALID, "out is null");
+  *out = nullptr;
+  if (n_instruments <= 0) return fail(MLB_ERR_INVALID, "n_instruments must be positive (got %d)", n_instruments);
+  if (!(sample_rate > 0.f)) return fail(MLB_ERR_INVALID, "sample_rate must be positive (got %g)", sample_rate);
+  if (protocol != 0 && protocol != 1) return fail(MLB_ERR_INVALID, "protocol must be 0 (MIDI) or 1 (MPE), got %d", protocol);
+  if (!controllers) return fail(MLB_ERR_INVALID, "null controller list");
+  if (n_controllers < 1 || n_controllers > 129)
+    return fail(MLB_ERR_INVALID, "n_controllers must be in 1..129 (got %d)", n_controllers);
+  int seen[129];
+  std::fill_n(seen, 129, -1);
+  for (int k = 0; k < n_controllers; ++k)
+  {
+    const int n = controllers[k];
+    if (n < 0 || n > 128) return fail(MLB_ERR_INVALID, "controller %d (list index %d) is not in 0..128", n, k);
+    if (seen[n] >= 0)
+      return fail(MLB_ERR_INVALID, "controller %d is requested twice (list indexes %d and %d)", n, seen[n], k);
+    seen[n] = k;
+  }
+  MLB_TRY(ensure_init());
+  std::unique_ptr<mlb_controllers> cb(new mlb_controllers);
+  cb->live.arm();
+  cb->G = n_instruments, cb->C = n_controllers, cb->protocol = protocol;
+  // SmoothedController::process (.cpp:274-285): int glideTimeInSamples = sr * kControllerGlideTimeSeconds in double
+  float c[2];
+  mlb_coeffs_glide((float)(int)((double)sample_rate * (double)0.02f), c);
+  cb->per_f = c[0], cb->dy = c[1];
+  const size_t CG = (size_t)n_controllers * n_instruments;
+  MLB_TRY(cb->d_ctrl.alloc((size_t)n_controllers * 4, "controller list"));
+  MLB_TRY(cb->d_state.alloc((size_t)CS_COUNT * CG * 4, "controller bank"));
+  MLB_TRY(cb->d_rows.alloc(CG * MLB_BLOCK * 4, "controller bank"));
+  CU_CHECK(cudaMemcpy(cb->d_ctrl.get(), controllers, (size_t)n_controllers * 4, cudaMemcpyHostToDevice));
+  MLB_TRY(mlb_controllers_clear(cb.get()));
+  MLB_TRY(cb->stream.create(cudaStreamNonBlocking));
+  *out = cb.release();
+  return MLB_OK;
+}
+
+extern "C" int mlb_controllers_get_state(mlb_controllers* cb, uint32_t* words, float* rows)
+{
+  if (!cb || !words || !rows) return fail(MLB_ERR_INVALID, "null argument");
+  const size_t CG = (size_t)cb->C * cb->G;
+  CU_CHECK(cudaMemcpy(words, cb->d_state.get(), (size_t)CS_COUNT * CG * 4, cudaMemcpyDeviceToHost));
+  CU_CHECK(cudaMemcpy(rows, cb->d_rows.get(), CG * MLB_BLOCK * 4, cudaMemcpyDeviceToHost));
+  for (size_t s = 0; s < CG; ++s)  // an idle glide's row is its target (not kept in device memory)
+    if ((int32_t)words[CS_REM * CG + s] < 0)
+    {
+      float tgt;
+      memcpy(&tgt, &words[CS_TARGET * CG + s], 4);
+      std::fill_n(rows + s * MLB_BLOCK, MLB_BLOCK, tgt);
+    }
+  return MLB_OK;
+}
+
+extern "C" int mlb_controllers_set_state(mlb_controllers* cb, const uint32_t* words, const float* rows)
+{
+  if (!cb || !words || !rows) return fail(MLB_ERR_INVALID, "null argument");
+  const size_t CG = (size_t)cb->C * cb->G;
+  CU_CHECK(cudaMemcpy(cb->d_state.get(), words, (size_t)CS_COUNT * CG * 4, cudaMemcpyHostToDevice));
+  CU_CHECK(cudaMemcpy(cb->d_rows.get(), rows, CG * MLB_BLOCK * 4, cudaMemcpyHostToDevice));
+  return MLB_OK;
+}
+
+extern "C" int mlb_controllers_set_voice_map(mlb_controllers* cb, const int32_t* voice_instrument, int n_voices)
+{
+  if (!cb) return fail(MLB_ERR_INVALID, "null controller bank");
+  if (!voice_instrument)
+  {
+    cb->d_vmap.reset();
+    cb->V = 0;
+    return MLB_OK;
+  }
+  if (n_voices <= 0) return fail(MLB_ERR_INVALID, "n_voices must be positive (got %d)", n_voices);
+  const int G = cb->G;
+  std::vector<int32_t> tab((size_t)G + 2 + n_voices, 0);  // counting sort by instrument, the unmapped (-1) ones last
+  for (int v = 0; v < n_voices; ++v)
+  {
+    const int g = voice_instrument[v];
+    if (g < -1 || g >= G)
+      return fail(MLB_ERR_INVALID, "voice %d: instrument %d is not -1 or one of the %d instruments", v, g, G);
+    ++tab[(g < 0 ? G : g) + 1];
+  }
+  for (int g = 0; g <= G; ++g) tab[g + 1] += tab[g];
+  std::vector<int32_t> fill(tab.begin(), tab.begin() + G + 1);
+  for (int v = 0; v < n_voices; ++v)
+  {
+    const int g = voice_instrument[v] < 0 ? G : voice_instrument[v];
+    tab[(size_t)G + 2 + fill[g]++] = v;
+  }
+  MLB_TRY(cb->d_vmap.alloc(tab.size() * 4, "voice map"));
+  CU_CHECK(cudaMemcpy(cb->d_vmap.get(), tab.data(), tab.size() * 4, cudaMemcpyHostToDevice));
+  cb->V = n_voices;
+  return MLB_OK;
+}
+
+extern "C" int mlb_controllers_process_device(mlb_controllers* cb, const int32_t* offsets_dev,
+                                              const mlb_controller_change* changes_dev, float* out_dev, int plane0,
+                                              int n_planes, int n_blocks, void* stream)
+{
+  if (!cb || !offsets_dev || !out_dev) return fail(MLB_ERR_INVALID, "null argument");
+  if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive (got %d)", n_blocks);
+  if (plane0 < 0 || n_planes < plane0 + cb->C)
+    return fail(MLB_ERR_INVALID, "planes [%d, %d) of the %d controllers are not within the %d output planes", plane0,
+                plane0 + cb->C, cb->C, n_planes);
+  CtrlArgs a;
+  a.offsets = offsets_dev, a.changes = changes_dev, a.ctrl = cb->d_ctrl.get();
+  a.state = cb->d_state.get(), a.rows = cb->d_rows.get(), a.out = out_dev;
+  a.vmap_off = cb->V ? cb->d_vmap.get() : nullptr;
+  a.vmap_voice = cb->V ? cb->d_vmap.get() + cb->G + 2 : nullptr;
+  a.G = cb->G, a.C = cb->C, a.N = cb->V ? cb->V : cb->G, a.T = n_blocks;
+  a.plane0 = plane0, a.n_planes = n_planes;
+  a.n_gblk = (cb->G + 31) / 32;
+  a.per_f = cb->per_f, a.dy = cb->dy;
+  const long long n_warps = (long long)a.C * a.n_gblk;
+  controller_bank_kernel<<<(unsigned)((n_warps + kCtrlWarps - 1) / kCtrlWarps), 32 * kCtrlWarps, 0,
+                           (cudaStream_t)stream>>>(a);
+  ++g_launches;
+  CU_CHECK(cudaGetLastError());
+  return MLB_OK;
+}
+
+// offsets [T][G + 1] must index changes of n_changes entries, non-decreasing within each block
+static int controllers_check_offsets(const mlb_controllers* cb, const int32_t* offsets, int n_changes, int n_blocks)
+{
+  for (int t = 0; t < n_blocks; ++t)
+  {
+    const int32_t* o = offsets + (size_t)t * (cb->G + 1);
+    for (int g = 0; g < cb->G; ++g)
+      if (o[g] < 0 || o[g] > o[g + 1] || o[g + 1] > n_changes)
+        return fail(MLB_ERR_INVALID, "block %d, instrument %d: change range [%d, %d) is not within the %d changes", t,
+                    g, o[g], o[g + 1], n_changes);
+  }
+  return MLB_OK;
+}
+
+extern "C" int mlb_controllers_process_host(mlb_controllers* cb, const int32_t* offsets_host,
+                                            const mlb_controller_change* changes_host, int n_changes, float* out_host,
+                                            int plane0, int n_planes, int n_blocks)
+{
+  if (!cb || !offsets_host || !out_host || (n_changes > 0 && !changes_host)) return fail(MLB_ERR_INVALID, "null argument");
+  if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive (got %d)", n_blocks);
+  if (n_changes < 0) return fail(MLB_ERR_INVALID, "n_changes must not be negative (got %d)", n_changes);
+  MLB_TRY(controllers_check_offsets(cb, offsets_host, n_changes, n_blocks));
+  if (plane0 < 0 || n_planes < plane0 + cb->C)
+    return fail(MLB_ERR_INVALID, "planes [%d, %d) of the %d controllers are not within the %d output planes", plane0,
+                plane0 + cb->C, cb->C, n_planes);
+  const size_t T = (size_t)n_blocks, N = cb->V ? cb->V : cb->G;
+  const size_t off_bytes = T * (cb->G + 1) * 4, ch_bytes = (size_t)n_changes * sizeof(mlb_controller_change);
+  const size_t out_bytes = T * n_planes * N * MLB_BLOCK * 4;
+  MLB_TRY(cb->d_off.ensure(off_bytes, "staging"));
+  if (n_changes) MLB_TRY(cb->d_ch.ensure(ch_bytes, "staging"));
+  MLB_TRY(cb->d_out.ensure(out_bytes, "staging"));
+  cudaStream_t s = cb->stream.get();
+  const int rc = [&]() -> int
+  {
+    CU_CHECK(cudaMemcpyAsync(cb->d_off.get(), offsets_host, off_bytes, cudaMemcpyHostToDevice, s));
+    if (n_changes) CU_CHECK(cudaMemcpyAsync(cb->d_ch.get(), changes_host, ch_bytes, cudaMemcpyHostToDevice, s));
+    MLB_TRY(mlb_controllers_process_device(cb, cb->d_off.get(), cb->d_ch.get(), cb->d_out.get(), plane0, n_planes,
+                                           n_blocks, s));
+    // only the controller planes come down: the caller's other planes stay as they were
+    const size_t plane = N * MLB_BLOCK * 4, pitch = (size_t)n_planes * plane;
+    CU_CHECK(cudaMemcpy2DAsync(reinterpret_cast<char*>(out_host) + plane0 * plane, pitch,
+                               reinterpret_cast<const char*>(cb->d_out.get()) + plane0 * plane, pitch, cb->C * plane, T,
+                               cudaMemcpyDeviceToHost, s));
+    return MLB_OK;
+  }();
+  return drain(rc, {s});
+}
+
+// Contract E with controller planes: the graph's input per block is the 8 Voice rows, then the C controller rows
+// in the bank's list order.  Per time chunk on the pipeline of mlb_synth_process_host: records and offsets go up on
+// s_h2d (all changes with the first chunk), the voice kernel, K11 and the graph run on the graph's stream, output rows
+// come down on s_d2h.
+extern "C" int mlb_synth_process_controllers_host(mlb_voices* vb, mlb_controllers* cb, mlb_graph* g,
+                                                  const mlb_voice_events* events_host, const int32_t* ctrl_offsets_host,
+                                                  const mlb_controller_change* ctrl_changes_host, float* out_host,
+                                                  float* mix_host, int n_blocks)
+{
+  if (!cb || !ctrl_offsets_host) return fail(MLB_ERR_INVALID, "null argument");
+  const int n_planes = MLB_VOICE_ROWS + cb->C;
+  unsigned row_mask;
+  MLB_TRY(synth_check(vb, g, events_host, n_blocks, out_host || mix_host, &row_mask, n_planes));
+  if (cb->V != g->V)
+    return fail(MLB_ERR_INVALID, "controller bank's voice map has %d voices, graph has %d (mlb_controllers_set_voice_map)",
+                cb->V, g->V);
+  if ((cb->protocol == 0) != ((vb->flags & MLB_VOICES_MIDI) != 0))
+    return fail(MLB_ERR_INVALID, "controller bank protocol %s, voice bank %s MLB_VOICES_MIDI", cb->protocol ? "MPE" : "MIDI",
+                (vb->flags & MLB_VOICES_MIDI) ? "with" : "without");
+  int n_changes = 0;  // the changes the offsets index
+  for (int t = 0; t < n_blocks; ++t) n_changes = std::max(n_changes, ctrl_offsets_host[(size_t)t * (cb->G + 1) + cb->G]);
+  if (n_changes > 0 && !ctrl_changes_host) return fail(MLB_ERR_INVALID, "null controller changes");
+  MLB_TRY(controllers_check_offsets(cb, ctrl_offsets_host, n_changes, n_blocks));
+  MLB_TRY(ensure_init());
+  const size_t V = (size_t)g->V, T = (size_t)n_blocks, n_out = g->outs.size(), G1 = (size_t)cb->G + 1;
+  const int Tc = synth_chunk_blocks(g, n_blocks, n_planes);
+  if (out_host) MLB_TRY(g->d_out.ensure(T * n_out * V * MLB_BLOCK * 4, "staging"));
+  if (mix_host) MLB_TRY(g->d_mix.ensure(T * n_out * MLB_BLOCK * 4, "staging"));
+  MLB_TRY(vb->d_ev.ensure(T * V * sizeof(mlb_voice_events), "staging"));
+  MLB_TRY(vb->d_out.ensure((size_t)Tc * n_planes * V * MLB_BLOCK * 4, "staging"));
+  MLB_TRY(cb->d_off.ensure(T * G1 * 4, "staging"));
+  if (n_changes) MLB_TRY(cb->d_ch.ensure((size_t)n_changes * sizeof(mlb_controller_change), "staging"));
+  const size_t row_floats = n_out * V * MLB_BLOCK;  // output rows per block
+  const int rc = [&]() -> int
+  {
+    MLB_TRY(host_pipeline(
+        g, n_blocks, Tc, true, out_host != nullptr,
+        [&](int t0, int t1, cudaStream_t s)
+        {
+          cudaError_t e = cudaSuccess;
+          if (t0 == 0 && n_changes)
+            e = cudaMemcpyAsync(cb->d_ch.get(), ctrl_changes_host, (size_t)n_changes * sizeof(mlb_controller_change),
+                                cudaMemcpyHostToDevice, s);
+          if (e == cudaSuccess)
+            e = cudaMemcpyAsync(cb->d_off.get() + t0 * G1, ctrl_offsets_host + t0 * G1, (t1 - t0) * G1 * 4,
+                                cudaMemcpyHostToDevice, s);
+          if (e == cudaSuccess)
+            e = cudaMemcpyAsync(vb->d_ev.get() + t0 * V, events_host + t0 * V, (t1 - t0) * V * sizeof(mlb_voice_events),
+                                cudaMemcpyHostToDevice, s);
+          return e;
+        },
+        [&](int t0, int t1, cudaStream_t s) -> int
+        {
+          MLB_TRY(voices_launch(vb, vb->d_ev.get() + t0 * V, vb->d_out.get(), t1 - t0, row_mask, n_planes, s));
+          MLB_TRY(mlb_controllers_process_device(cb, cb->d_off.get() + t0 * G1, cb->d_ch.get(), vb->d_out.get(),
+                                                 MLB_VOICE_ROWS, n_planes, t1 - t0, s));
+          return graph_process(g, vb->d_out.get(), n_planes, out_host ? g->d_out.get() + t0 * row_floats : nullptr,
+                               mix_host ? g->d_mix.get() + t0 * n_out * MLB_BLOCK : nullptr, t1 - t0, s);
+        },
+        [&](int t0, int t1, cudaStream_t s)
+        {
+          return cudaMemcpyAsync(out_host + t0 * row_floats, g->d_out.get() + t0 * row_floats,
+                                 (t1 - t0) * row_floats * 4, cudaMemcpyDeviceToHost, s);
+        }));
+    if (mix_host) MLB_TRY(mlb_graph_mix_wait(g, g->stream.get()));
+    if (mix_host)
+      CU_CHECK(cudaMemcpyAsync(mix_host, g->d_mix.get(), T * n_out * MLB_BLOCK * 4, cudaMemcpyDeviceToHost, g->stream.get()));
+    return MLB_OK;
+  }();
   return drain(rc, {g->s_h2d.get(), g->stream.get(), g->s_d2h.get()});
 }
 
@@ -2935,4 +3232,11 @@ extern "C" int mlb_router_process_vector(mlb_router* r, int start_time, mlb_voic
 {
   if (!r || !records) return -1;
   return r->router.processVector(start_time, records);
+}
+extern "C" int mlb_router_controller_changes(const mlb_router* r, mlb_controller_change* out, int cap)
+{
+  if (!r || (cap > 0 && !out)) return -1;
+  const std::vector<mlb_controller_change>& c = r->router.controllerChanges();
+  std::copy_n(c.begin(), std::min<size_t>(c.size(), (size_t)std::max(cap, 0)), out);
+  return (int)c.size();
 }

@@ -26,7 +26,8 @@ enum VoiceCoef { VC_GLIDE_SAMPLES = 0, VC_DRIFT_AMOUNT, VC_BEND_RANGE, VC_VOICE_
 struct VoiceArgs
 {
   const mlb_voice_events* ev;  // [T][V]
-  float* out;                  // [T][8][V][64]
+  float* out;                  // [T][P][V][64], rows in planes 0..7
+  size_t out_block;            // floats per block of out: P * V * 64 (P = 8, or more when controller planes follow)
   uint32_t* state;             // [VS_COUNT][V]
   const float* coef;           // [VC_COUNT][V]
   float* grows;                // [VG_COUNT][V][64]  LinearGlide::mCurrVec
@@ -570,7 +571,7 @@ __global__ void __launch_bounds__(32 * (TIME ? kVoiceWarpsPerCtaTime : kVoiceWar
       gp[i] = o.g;
       if (live) gw[0] = o.s0, gw[V] = o.s1, gw[2 * V] = o.s2;
     }
-    float* const planes = a.out + (size_t)t * MLB_VOICE_ROWS * V * MLB_BLOCK;
+    float* const planes = a.out + (size_t)t * a.out_block;
     const size_t plane_floats = V * MLB_BLOCK;
     GlideLane gl[VG_COUNT];
 #pragma unroll
@@ -685,9 +686,9 @@ __global__ void __launch_bounds__(32 * (TIME ? kVoiceWarpsPerCtaTime : kVoiceWar
 }
 
 // processVector's MPE tail (E:448-460): pitch, x, y, z, mod rows += the rows of the instrument's main voice.
-// One thread per float4 of a (block, voice) row; planes [T][8][V][64].
+// One thread per float4 of a (block, voice) row; planes [T][n_planes][V][64].
 __global__ void __launch_bounds__(256) voice_mpe_add_kernel(float* out, const int32_t* main_voice, int V, int T,
-                                                             unsigned row_mask)
+                                                             unsigned row_mask, int n_planes)
 {
   const size_t n4 = (size_t)T * V * 16;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x)
@@ -703,7 +704,7 @@ __global__ void __launch_bounds__(256) voice_mpe_add_kernel(float* out, const in
     for (int k = 0; k < 5; ++k)
     {
       if (!((row_mask >> rows[k]) & 1u)) continue;
-      float4* plane = reinterpret_cast<float4*>(out + (t * MLB_VOICE_ROWS + rows[k]) * (size_t)V * MLB_BLOCK);
+      float4* plane = reinterpret_cast<float4*>(out + (t * n_planes + rows[k]) * (size_t)V * MLB_BLOCK);
       float4 a = plane[(size_t)v * 16 + q];
       const float4 b = plane[(size_t)m * 16 + q];
       a.x = __fadd_rn(a.x, b.x), a.y = __fadd_rn(a.y, b.y), a.z = __fadd_rn(a.z, b.z), a.w = __fadd_rn(a.w, b.w);

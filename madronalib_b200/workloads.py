@@ -696,6 +696,39 @@ def instrument_buses(n_instruments: int, polyphony: int, mpe: bool = False):
     return first, np.full(n_instruments, polyphony, np.int32)
 
 
+CONTROLLER_POOL = (1, 2, 7, 10, 11, 16, 64, 71, 73, 74, 128)  # mod wheel, breath, volume, pan, expression, ...
+
+
+def controller_changes(n_instruments: int, n_blocks: int, density: float = 0.05, seed: int = 11,
+                       pool=CONTROLLER_POOL):
+    """A MIDI-fader-like controller stream for api.ControllerBank: in a fraction `density` of the (block, instrument)
+    pairs a fader moves, sending 1 to 4 writes in the block, mostly to one controller of `pool` (so that some
+    blocks hold several writes to one controller, the last of which counts) with 7-bit values (k / 127) walking
+    from where the fader was.  Returns (offsets [T][G + 1] int32, changes of api.CONTROLLER_CHANGE_DTYPE)."""
+    from .api import CONTROLLER_CHANGE_DTYPE
+    rng = np.random.default_rng(seed)
+    G, T = int(n_instruments), int(n_blocks)
+    pool = np.asarray(pool, np.uint16)
+    n = np.where(rng.random((T, G)) < density, rng.integers(1, 5, (T, G)), 0)
+    offsets = np.zeros((T, G + 1), np.int32)
+    ends = np.cumsum(n.ravel()).reshape(T, G)
+    offsets[:, 1:] = ends
+    offsets[:, 0] = np.concatenate(([0], ends[:-1, -1]))
+    total = int(n.sum())
+    burst = np.repeat(np.arange(n.size), n.ravel())                # the (block, instrument) pair of each write
+    fader = rng.integers(0, len(pool), n.size)[burst]               # the burst's controller ...
+    other = rng.random(total) < 0.25                                 # ... or, now and then, another one
+    ctrl = np.where(other, rng.integers(0, len(pool), total), fader)
+    start = rng.integers(0, 128, n.size)[burst]
+    pos = np.arange(total) - np.repeat(np.cumsum(n.ravel()) - n.ravel(), n.ravel())
+    step = rng.integers(-6, 7, n.size)[burst]
+    value = np.clip(start + pos * step, 0, 127).astype(np.float32) / np.float32(127)
+    changes = np.zeros(total, CONTROLLER_CHANGE_DTYPE)
+    changes["controller"] = pool[ctrl]
+    changes["value"] = value
+    return offsets, changes
+
+
 # ---- random voice graphs (tests): any DAG of the op table, for checker-vs-checker and GPU-vs-checker runs ----
 
 def random_graph_workload(seed: int, n_voices: int = 37, n_nodes: int = 24, hw_approx: bool = True,

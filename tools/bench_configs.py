@@ -2,7 +2,7 @@
 """Kernel-resident timing of everything except the headline: BASELINE.json configurations 2-5, the
 SURVEY 8(f) workloads (config 6 = Aaltoverb x V, the EventsToSignals::Voice bank) and the elementwise maps.
 
-    python tools/bench_configs.py [--steps K] [--only 2,3,4,5,6,voices,map,fdtd,buses] [--generic] [--cpu]
+    python tools/bench_configs.py [--steps K] [--only 2,3,4,5,6,voices,map,fdtd,buses,controllers] [--generic] [--cpu]
 
 Prints one JSON line per configuration: kernel name, mean CUDA-event kernel time, algorithmic
 bytes per launch (SURVEY.md 8d / DESIGN.md), achieved GB/s and fraction of the measured HBM peak.
@@ -29,7 +29,7 @@ def main():
     from madronalib_b200 import api, workloads as wl
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
-    ap.add_argument("--only", default="2,3,swept,4,5,6,voices,map,fdtd,buses")
+    ap.add_argument("--only", default="2,3,swept,4,5,6,voices,map,fdtd,buses,controllers")
     ap.add_argument("--generic", action="store_true", help="force the graph interpreter kernel")
     ap.add_argument("--cpu", action="store_true",
                     help="also time the reference (oracle/_ref, all host threads) on config 6, the Voice bank "
@@ -120,6 +120,8 @@ def main():
         bench_fdtd(api, wl, torch, dev, args.steps, args.cpu)
     if "buses" in only:
         bench_buses(api, wl, torch, dev, args.steps)
+    if "controllers" in only:
+        bench_controllers(api, wl, torch, dev, args.steps)
     if args.cpu:
         # the reference itself on this box's host cores (oracle/_ref; checker code, used here only as a baseline)
         import time
@@ -379,6 +381,91 @@ def bench_contract_e_buses(api, wl, torch, facts, n_calls=5):
     print(json.dumps({"config": "contract_E_buses_parity", "buses": int(len(sel)), "blocks": T,
                       "calls_replayed": calls, "checker": "port bank -> port graph -> port buses",
                       "mismatches": mism}), flush=True)
+
+
+def bench_controllers(api, wl, torch, dev, steps):
+    """K11 alone, change lists resident on the device: 4 096 instruments x 129 and x 9 controllers x 64 vectors of
+    fader moves (density 0.05), mean of `steps` CUDA-event-timed launches after 3 warm-up launches.  Bytes written =
+    the controller rows (the bound: idle rows are stored without being read).  Parity of 16 sampled instruments of
+    the first launch against the plain-C port.  Then contract E at 65 536 voices x 64 vectors of config A with 4
+    controller planes (4 096 instruments x 16 voices), host clock around calls that return finished."""
+    import time
+    from oracle import ctrl_bindings as cbind
+    T, G = 64, 4096
+    facts = gpu_facts()
+    offsets, ch = wl.controller_changes(G, T, density=0.05, seed=40)
+    d_off = torch.from_numpy(offsets).to(dev)
+    d_ch = torch.from_numpy(ch.view(np.int64)).to(dev)
+    sel = np.linspace(0, G - 1, 16).astype(np.int64)
+    for C in (129, 9):
+        ctrl = list(range(129)) if C == 129 else list(wl.CONTROLLER_POOL[:9])
+        out = torch.empty((T, C, G, 64), dtype=torch.float32, device=dev)
+        bank = api.ControllerBank(G, ctrl, 48000.0)
+        sh = torch.cuda.current_stream().cuda_stream
+        bank.process_device(d_off, d_ch, out, T, stream=sh)
+        torch.cuda.synchronize()
+        got = out[:, :, torch.from_numpy(sel).to(dev)].cpu().numpy()
+        for _ in range(2):
+            bank.process_device(d_off, d_ch, out, T, stream=sh)
+        times = []
+        for _ in range(steps):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            bank.process_device(d_off, d_ch, out, T, stream=sh)
+            e1.record()
+            torch.cuda.synchronize()
+            times.append(e0.elapsed_time(e1))
+        bank.close()
+        sub_off = np.zeros((T, len(sel) + 1), np.int32)
+        parts, n = [], 0
+        for t in range(T):
+            for j, g in enumerate(sel):
+                sub_off[t, j] = n
+                parts.append(ch[offsets[t, g]:offsets[t, g + 1]])
+                n += parts[-1].size
+            sub_off[t, -1] = n
+        want, _, _ = cbind.port_controllers(len(sel), ctrl, sub_off, np.concatenate(parts), 48000.0)
+        mism = int(((got.view(np.uint32) != want.view(np.uint32)) & ~(np.isnan(got) & np.isnan(want))).sum())
+        ms = float(np.mean(times))
+        nbytes = 256.0 * T * C * G
+        print(json.dumps({
+            "config": "controllers_%dx%d" % (G, C), "kernel": "controller_bank_kernel", "instruments": G,
+            "controllers": C, "blocks": T, "changes": int(ch.size), "kernel_ms": ms, "bytes_written": nbytes,
+            "achieved_gbs": nbytes / (ms * 1e-3) / 1e9,
+            "frac_of_datasheet_hbm": nbytes / (ms * 1e-3) / 1e9 / HBM_DATASHEET_GBS,
+            "datasheet_note": "3.35 TB/s, H100 SXM data sheet", **facts,
+            "parity_instruments": int(len(sel)), "parity_checker": "plain-C port", "mismatches": mism}), flush=True)
+        del out
+        torch.cuda.empty_cache()
+    del d_off, d_ch
+    V, poly, n_calls = 65536, 16, 5
+    ctrl = [1, 7, 11, 128]
+    w = wl.config_a(V)
+    prm = wl.synth_bank_params(V)
+    ev_np = wl.synth_events(V, T)
+    h_ev = torch.empty(ev_np.nbytes, dtype=torch.uint8).pin_memory()
+    h_ev.numpy()[:] = ev_np.view(np.uint8).reshape(-1)
+    ev = h_ev.numpy().view(ev_np.dtype).reshape(T, V)
+    vb = api.VoiceBank(48000.0, *prm)
+    cb = api.ControllerBank(V // poly, ctrl, 48000.0, protocol=api.ControllerBank.MPE)
+    cb.set_voice_map(np.repeat(np.arange(V // poly, dtype=np.int32), poly))
+    offsets, ch = wl.controller_changes(V // poly, T, density=0.05, seed=41, pool=ctrl)
+    g = api.VoiceGraph(w.spec, V)
+    g.set_coefs(w.coef)
+    g.set_state(w.state)
+    g.process_events_controllers_host(vb, cb, ev, offsets, ch, want_out=False, want_mix=True)
+    t0 = time.perf_counter()
+    for _ in range(n_calls):
+        g.process_events_controllers_host(vb, cb, ev, offsets, ch, want_out=False, want_mix=True)
+    dt = time.perf_counter() - t0
+    print(json.dumps({"config": "contract_E_controllers_mix", "voices": V, "blocks": T, "controller_planes": len(ctrl),
+                      "ms_per_call": 1e3 * dt / n_calls, "voice_samples_per_s": V * T * 64 * n_calls / dt,
+                      "h2d_bytes_per_call": int(ev.nbytes + offsets.nbytes + ch.nbytes),
+                      "time_chunks": g.last_host_slices,
+                      "kernels": "voice_bank_kernel -> controller_bank_kernel -> " + g.kernel_name, **facts}),
+          flush=True)
+    for h in (g, vb, cb):
+        h.close()
 
 
 if __name__ == "__main__":
