@@ -687,6 +687,63 @@ int mlb_synth_process_controllers_host(mlb_voices* vb, mlb_controllers* cb, mlb_
                                        const mlb_controller_change* ctrl_changes_host, float* out_host,
                                        float* mix_host, int n_blocks);
 
+/* ---- Event routing of G instruments on the device (K12) ----------------------------------------
+ * Per instrument g and block t, a router bank produces exactly what one mlb_router (mlb::VoiceRouter) with the same
+ * settings produces after the same mlb_router_add_event calls and mlb_router_process_vector(t * 64): the records,
+ * byte for byte; the controller writes, in the order of mlb_router_controller_changes; the overflow and unsupported
+ * counts.  Routing state carries over from call to call.
+ * Input per block t: the events of instrument g are events[offsets[t][g] .. offsets[t][g + 1]) (offsets [T][G + 1]
+ * int32, the CSR convention of mlb_controllers_process_*), in arrival order, with mlb_event.time the frame within the
+ * block (0..63).  Instrument g writes its mlb_router_record_count() records to voices first_voice[g] ..: polyphony
+ * records in MIDI, polyphony + 1 in MPE with the main voice first (workloads.instrument_buses' layout); every voice of
+ * no instrument gets an all-zero record.  Output: records [T][V], the buffer mlb_voices_process_* reads, and the
+ * controller writes as change_offsets [T][G + 1] into changes, which mlb_controllers_process_* consume as they are
+ * (each event makes at most one write, so changes needs room for one per event range entry the offsets reference). */
+typedef struct mlb_routers mlb_routers;
+/* polyphony[g] in 0..16, first_voice[g] (ranges [first, first + record count) within [0, n_voices), not
+ * overlapping); unison[g] 0/1 and mod_cc[g] in 0..128 (EventsToSignals::setModCC) may be NULL (off, 16).  protocol:
+ * 0 MIDI, 1 MPE, for every instrument.  Arguments are validated on the host; MLB_ERR_INVALID names the offending
+ * instrument.  A live bank counts toward mlb_init's one-device rule. */
+int mlb_routers_create(int n_instruments, int protocol, const int32_t* polyphony, const int32_t* first_voice,
+                       const int32_t* unison, const int32_t* mod_cc, int n_voices, mlb_routers** out);
+int mlb_routers_destroy(mlb_routers* r);
+/* every instrument back to its state right after create (voices, keys, pedal, note-on counter); counters kept.
+ * Ordered after this bank's host calls; a caller of mlb_routers_process_device synchronises its stream first. */
+int mlb_routers_clear(mlb_routers* r);
+/* per instrument, since create: note events that found their voice's record full (MLB_VOICE_MAX_EVENTS per voice and
+ * vector; the sum of mlb_router_process_vector's returns), and CC 120 events with value 0 (not routed).  Either
+ * pointer may be NULL.  Ordered as mlb_routers_clear. */
+int mlb_routers_counters(mlb_routers* r, int64_t* overflow, int64_t* unsupported);
+/* three launches for n_blocks vectors, no allocation, no synchronisation (capturable into a CUDA graph).  The device
+ * path does not check its input: event times must be in 0..63, offsets within the events. */
+int mlb_routers_process_device(mlb_routers* r, const int32_t* offsets_dev, const mlb_event* events_dev,
+                               mlb_voice_events* records_dev, int32_t* change_offsets_dev,
+                               mlb_controller_change* changes_dev, int n_blocks, void* stream);
+/* host buffers: offsets (non-decreasing per block, within [0, n_events]) and the times of the events they reference
+ * are checked before anything is copied; records_host [T][V], change_offsets_host [T][G + 1], changes_host with room
+ * for changes_capacity writes.  The writes are counted over every range the offsets reference (a range referenced
+ * twice counts twice); more than changes_capacity is refused before anything is copied.  *n_changes_out (may be NULL)
+ * = the writes made.  Returns when its copies are finished. */
+int mlb_routers_process_host(mlb_routers* r, const int32_t* offsets_host, const mlb_event* events_host, int n_events,
+                             mlb_voice_events* records_host, int32_t* change_offsets_host,
+                             mlb_controller_change* changes_host, int changes_capacity, int* n_changes_out,
+                             int n_blocks);
+/* the controller writes the events of offsets_host make, counted as mlb_routers_process_host counts them (after the
+ * same checks); the capacity its changes_host needs */
+int mlb_routers_count_changes(mlb_routers* r, const int32_t* offsets_host, const mlb_event* events_host, int n_events,
+                              int n_blocks, int* n_changes_out);
+/* Contract E from raw events: per time chunk on the pipeline of mlb_synth_process_host, the offsets go up (all events
+ * with the first chunk), then K12 -> the voice bank -> the controller bank (if given) -> the graph -> the bus sum (if
+ * buses are given) or the mix bus; the records and change lists never leave the device.  The graph's input is the 8
+ * Voice rows, then the controller planes when a controller bank is given, as in the other contract-E entry points.
+ * Without buses: out_host [T][n_out][V][64] and / or mix_host [T][n_out][64] (either may be NULL), bus_host NULL;
+ * with buses: bus_host [T][n_out][G_bus][64], out_host and mix_host NULL.  MLB_ERR_INVALID, before anything is copied,
+ * names the mismatch: voice counts of the routers, voice bank, graph, buses and controller voice map; the routers'
+ * protocol against the voice bank's MLB_VOICES_MIDI flag or the controller bank's; bad offsets or event times. */
+int mlb_synth_process_routed_host(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb, mlb_graph* g, mlb_buses* b,
+                                  const int32_t* offsets_host, const mlb_event* events_host, int n_events,
+                                  float* out_host, float* mix_host, float* bus_host, int n_blocks);
+
 #ifdef __cplusplus
 }
 #endif

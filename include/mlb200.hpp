@@ -760,6 +760,63 @@ inline void processEventsWithControllers(VoiceBank& voices, ControllerBank& cont
                                            changes, out, mix, nBlocks));
 }
 
+// ---- RouterBank: the event routing of G instruments on the GPU (mlb_routers_*), what one mlb::VoiceRouter per
+// instrument produces: records, controller writes, overflow and unsupported counts ----
+class RouterBank
+{
+  mlb_routers* r_ = nullptr;
+  int instruments_ = 0, voices_ = 0;
+
+ public:
+  // protocol 0 MIDI, 1 MPE; polyphony[g] 0..16, firstVoice[g] (records at voices firstVoice[g] ..); unison and modCC
+  // may be nullptr (off, 16)
+  RouterBank(int nInstruments, int protocol, const int32_t* polyphony, const int32_t* firstVoice, int nVoices,
+             const int32_t* unison = nullptr, const int32_t* modCC = nullptr)
+      : instruments_(nInstruments), voices_(nVoices)
+  {
+    check(mlb_routers_create(nInstruments, protocol, polyphony, firstVoice, unison, modCC, nVoices, &r_));
+  }
+  ~RouterBank() { mlb_routers_destroy(r_); }
+  RouterBank(const RouterBank&) = delete;
+  RouterBank& operator=(const RouterBank&) = delete;
+  int instruments() const { return instruments_; }
+  int voices() const { return voices_; }
+  mlb_routers* handle() const { return r_; }
+  void clear() { check(mlb_routers_clear(r_)); }
+  // per instrument, since creation; either pointer may be nullptr
+  void counters(int64_t* overflow, int64_t* unsupported) { check(mlb_routers_counters(r_, overflow, unsupported)); }
+  // host buffers: offsets [nBlocks][instruments + 1] into events -> records [nBlocks][voices], changeOffsets
+  // [nBlocks][instruments + 1] into changes; returns the number of changes written
+  int process(const int32_t* offsets, const mlb_event* events, int nEvents, mlb_voice_events* records,
+              int32_t* changeOffsets, std::vector<mlb_controller_change>& changes, int nBlocks)
+  {
+    int n = 0;
+    check(mlb_routers_count_changes(r_, offsets, events, nEvents, nBlocks, &n));
+    changes.resize((size_t)n);
+    check(mlb_routers_process_host(r_, offsets, events, nEvents, records, changeOffsets, changes.data(), n, &n,
+                                   nBlocks));
+    return n;
+  }
+  // device buffers, asynchronous on `stream`: three launches, no allocation or synchronisation
+  void processDevice(const int32_t* offsets, const mlb_event* events, mlb_voice_events* records, int32_t* changeOffsets,
+                     mlb_controller_change* changes, int nBlocks, void* stream = nullptr)
+  {
+    check(mlb_routers_process_device(r_, offsets, events, records, changeOffsets, changes, nBlocks, stream));
+  }
+};
+
+// Contract E from raw events (mlb_synth_process_routed_host): offsets [nBlocks][instruments + 1] into events in,
+// routed, turned into Voice rows (and controller planes when `controllers` is given) and run through the graph on the
+// device.  Without buses: out / mix as processEvents; with buses: bus [nBlocks][n_out][buses][64].
+inline void processEventsRouted(RouterBank& routers, VoiceBank& voices, ControllerBank* controllers, DeviceBank& bank,
+                                Buses* buses, const int32_t* offsets, const mlb_event* events, int nEvents, float* out,
+                                float* mix, float* bus, int nBlocks)
+{
+  check(mlb_synth_process_routed_host(routers.handle(), voices.handle(), controllers ? controllers->handle() : nullptr,
+                                      bank.handle(), buses ? buses->handle() : nullptr, offsets, events, nEvents, out,
+                                      mix, bus, nBlocks));
+}
+
 // ---- Resampler: Upsampler(octaves) / Downsampler(octaves) x V on the GPU (mlb_resampler_*) ----
 class Resampler
 {

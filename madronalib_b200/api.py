@@ -119,6 +119,15 @@ def lib() -> ctypes.CDLL:
     L.mlb_buses_sum_device.argtypes = [_vp, _vp, _vp, ctypes.c_int, ctypes.c_int, _vp]
     L.mlb_synth_process_buses_host.argtypes = [_vp, _vp, _vp, _vp, _vp, ctypes.c_int]
     L.mlb_synth_process_controllers_host.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int]
+    L.mlb_routers_create.argtypes = [ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _vp, ctypes.c_int, _vp]
+    L.mlb_routers_destroy.argtypes = [_vp]
+    L.mlb_routers_clear.argtypes = [_vp]
+    L.mlb_routers_counters.argtypes = [_vp, _vp, _vp]
+    L.mlb_routers_process_device.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int, _vp]
+    L.mlb_routers_process_host.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp, _vp, _vp, ctypes.c_int, _vp, ctypes.c_int]
+    L.mlb_routers_count_changes.argtypes = [_vp, _vp, _vp, ctypes.c_int, ctypes.c_int, _vp]
+    L.mlb_synth_process_routed_host.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int, _vp, _vp, _vp,
+                                                ctypes.c_int]
     L.mlb_graph_process_host.argtypes = [_vp, _vp, _vp, _vp, ctypes.c_int]
     L.mlb_graph_last_kernel_ms.argtypes = [_vp, _vp]
     L.mlb_graph_last_host_slices.argtypes = [_vp]
@@ -452,6 +461,31 @@ class VoiceGraph(_Handle):
             raise ValueError(f"process_events_buses_host: `out` must be a C-contiguous float32 array of shape {shape}")
         _check(lib().mlb_synth_process_buses_host(bank._h, self._h, buses._h, events.ctypes.data, _ptr(out), T))
         return out
+
+    def process_routed_host(self, routers: "RouterBank", bank: "VoiceBank", offsets: np.ndarray, events: np.ndarray,
+                            controllers: Optional["ControllerBank"] = None, buses: Optional["Buses"] = None,
+                            want_out: bool = True, want_mix: bool = False):
+        """Contract E from raw events (mlb_synth_process_routed_host): offsets [T][G + 1] into events (EVENT_DTYPE) in,
+        routed on the device by ``routers``, then the Voice rows of ``bank``, the controller planes of ``controllers``
+        (if given) and this graph.  Without ``buses``: returns (out [T][n_out][V][64] or None, mix [T][n_out][64] or
+        None); with ``buses``: returns the bus rows [T][n_out][G_bus][64]."""
+        s, V = self.spec, self.n_voices
+        off = np.ascontiguousarray(offsets, np.int32)
+        if off.ndim != 2 or off.shape[1] != routers.n_instruments + 1:
+            raise ValueError(f"process_routed_host: offsets must be [T][{routers.n_instruments + 1}], got {off.shape}")
+        ev = np.ascontiguousarray(events, EVENT_DTYPE)
+        T = int(off.shape[0])
+        out = mix = bus = None
+        if buses is not None:
+            bus = np.empty((T, s.n_out, buses.n_buses, BLOCK), np.float32)
+        else:
+            out = np.empty((T, s.n_out, V, BLOCK), np.float32) if want_out else None
+            mix = np.empty((T, s.n_out, BLOCK), np.float32) if want_mix else None
+        _check(lib().mlb_synth_process_routed_host(routers._h, bank._h, controllers._h if controllers else None, self._h,
+                                                   buses._h if buses else None, off.ctypes.data,
+                                                   ev.ctypes.data if ev.size else None, int(ev.size), _ptr(out),
+                                                   _ptr(mix), _ptr(bus), T))
+        return bus if buses is not None else (out, mix)
 
     def process_device(self, inp, out, mix, n_blocks: int, stream: int = 0) -> None:
         """Device pointers (torch tensors / ints); asynchronous on ``stream`` (cudaStream_t)."""
@@ -793,3 +827,74 @@ class EventRouter(_Handle):
         if n:
             lib().mlb_router_controller_changes(self._h, out.ctypes.data, n)
         return out
+
+
+EVENT_DTYPE = np.dtype([("type", "u1"), ("channel", "u1"), ("source_idx", "<u2"), ("time", "<i4"),
+                        ("value1", "<f4"), ("value2", "<f4")])  # struct mlb_event
+assert EVENT_DTYPE.itemsize == 16
+
+
+class RouterBank(_Handle):
+    """The event routing of G instruments on the device (mlb_routers_*): per instrument and block, exactly what one
+    EventRouter with the same settings produces -- records, controller writes, overflow and unsupported counts.
+    Input per call: offsets [T][G + 1] into events (EVENT_DTYPE, arrival order, ``time`` the frame in the block).
+    Instrument g writes its records to voices first_voice[g] .. (polyphony[g] of them in MIDI, polyphony[g] + 1 in MPE
+    with the main voice first); a voice of no instrument gets an all-zero record."""
+
+    _destroy = "mlb_routers_destroy"
+
+    MIDI, MPE = 0, 1
+
+    def __init__(self, polyphony, first_voice, n_voices: int, protocol: int = 0, unison=None, mod_cc=None):
+        poly = np.ascontiguousarray(polyphony, np.int32)
+        first = np.ascontiguousarray(first_voice, np.int32)
+        if poly.ndim != 1 or poly.shape != first.shape:
+            raise ValueError(f"RouterBank: polyphony and first_voice must be 1-D of one length, got {poly.shape} and "
+                             f"{first.shape}")
+        uni = None if unison is None else np.ascontiguousarray(unison, np.int32)
+        mcc = None if mod_cc is None else np.ascontiguousarray(mod_cc, np.int32)
+        for name, a in (("unison", uni), ("mod_cc", mcc)):
+            if a is not None and a.shape != poly.shape:
+                raise ValueError(f"RouterBank: {name} must have one entry per instrument, got {a.shape}")
+        self.n_instruments, self.n_voices, self.protocol = int(poly.shape[0]), int(n_voices), int(protocol)
+        h = ctypes.c_void_p()
+        _check(lib().mlb_routers_create(self.n_instruments, self.protocol, poly.ctypes.data, first.ctypes.data,
+                                        None if uni is None else uni.ctypes.data,
+                                        None if mcc is None else mcc.ctypes.data, self.n_voices, ctypes.byref(h)))
+        self._h = h
+
+    def clear(self) -> None:
+        _check(lib().mlb_routers_clear(self._h))
+
+    def counters(self):
+        """(overflow [G], unsupported [G]) int64, since creation."""
+        ovf = np.zeros(self.n_instruments, np.int64)
+        uns = np.zeros(self.n_instruments, np.int64)
+        _check(lib().mlb_routers_counters(self._h, ovf.ctypes.data, uns.ctypes.data))
+        return ovf, uns
+
+    def process_host(self, offsets: np.ndarray, events: np.ndarray):
+        """-> (records [T][V] of workloads.VOICE_EVENTS_DTYPE, change_offsets [T][G + 1] int32, changes of
+        CONTROLLER_CHANGE_DTYPE)."""
+        from .workloads import VOICE_EVENTS_DTYPE
+        off = np.ascontiguousarray(offsets, np.int32)
+        if off.ndim != 2 or off.shape[1] != self.n_instruments + 1:
+            raise ValueError(f"process_host: offsets must be [T][{self.n_instruments + 1}], got {off.shape}")
+        ev = np.ascontiguousarray(events, EVENT_DTYPE)
+        T = int(off.shape[0])
+        rec = np.empty((T, self.n_voices), VOICE_EVENTS_DTYPE)
+        coff = np.empty((T, self.n_instruments + 1), np.int32)
+        n = ctypes.c_int(0)
+        evp = ev.ctypes.data if ev.size else None
+        # the writes are counted by the library over every referenced range (a range used twice counts twice)
+        _check(lib().mlb_routers_count_changes(self._h, off.ctypes.data, evp, int(ev.size), T, ctypes.byref(n)))
+        ch = np.zeros(max(n.value, 1), CONTROLLER_CHANGE_DTYPE)
+        _check(lib().mlb_routers_process_host(self._h, off.ctypes.data, evp, int(ev.size), rec.ctypes.data,
+                                              coff.ctypes.data, ch.ctypes.data, int(ch.size), ctypes.byref(n), T))
+        return rec, coff, ch[:n.value].copy()
+
+    def process_device(self, offsets, events, records, change_offsets, changes, n_blocks: int, stream: int = 0) -> None:
+        """Device buffers (torch tensors / ints); asynchronous on ``stream``, three kernel launches, no allocation or
+        synchronisation (capturable into a CUDA graph).  ``changes`` needs room for one write per event."""
+        _check(lib().mlb_routers_process_device(self._h, _ptr(offsets), _ptr(events), _ptr(records),
+                                                _ptr(change_offsets), _ptr(changes), int(n_blocks), stream or None))

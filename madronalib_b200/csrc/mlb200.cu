@@ -30,6 +30,7 @@
 #include "fdtd_kernel.cuh"
 #include "bus_kernel.cuh"
 #include "controller_kernel.cuh"
+#include "router_kernel.cuh"
 #include "generic_kernel.cuh"
 
 using namespace mlb;
@@ -2530,7 +2531,8 @@ extern "C" int mlb_voices_process_host(mlb_voices* vb, const mlb_voice_events* e
 
 // The checks both contract-E entry points share; *row_mask = the Voice rows the graph reads.
 // n_planes: the input planes per block, the 8 Voice rows and any controller planes after them.
-static int synth_check(const mlb_voices* vb, const mlb_graph* g, const mlb_voice_events* events_host, int n_blocks,
+// events_host: the records, or the raw events' offsets of the routed entry point.
+static int synth_check(const mlb_voices* vb, const mlb_graph* g, const void* events_host, int n_blocks,
                        bool wants_output, unsigned* row_mask, int n_planes = MLB_VOICE_ROWS)
 {
   if (!vb || !g || !events_host) return fail(MLB_ERR_INVALID, "null argument");
@@ -2974,6 +2976,305 @@ extern "C" int mlb_synth_process_controllers_host(mlb_voices* vb, mlb_controller
         {
           return cudaMemcpyAsync(out_host + t0 * row_floats, g->d_out.get() + t0 * row_floats,
                                  (t1 - t0) * row_floats * 4, cudaMemcpyDeviceToHost, s);
+        }));
+    if (mix_host) MLB_TRY(mlb_graph_mix_wait(g, g->stream.get()));
+    if (mix_host)
+      CU_CHECK(cudaMemcpyAsync(mix_host, g->d_mix.get(), T * n_out * MLB_BLOCK * 4, cudaMemcpyDeviceToHost, g->stream.get()));
+    return MLB_OK;
+  }();
+  return drain(rc, {g->s_h2d.get(), g->stream.get(), g->s_d2h.get()});
+}
+
+// ------------------------------------------------------------------------------------------
+// Event routing of G instruments (K12, router_kernel.cuh)
+
+struct mlb_routers
+{
+  // declared first, so released last: the buffers below are freed first, and cudaFree waits for the device
+  LiveCount live;
+  Stream stream;
+  int G = 0, V = 0, protocol = 0, n_unowned = 0;
+  DevBuf<int32_t> d_inst;     // [RI_COUNT][G]
+  DevBuf<int32_t> d_unowned;  // voices of no instrument
+  DevBuf<uint32_t> d_state;   // [G][kRouterWords][32]
+  DevBuf<int32_t> d_off, d_coff;  // staging of the host entry points
+  DevBuf<mlb_event> d_ev;
+  DevBuf<mlb_voice_events> d_rec;
+  DevBuf<mlb_controller_change> d_ch;
+};
+
+extern "C" int mlb_routers_destroy(mlb_routers* r)
+{
+  delete r;
+  return MLB_OK;
+}
+
+// the routing state right after VoiceRouter's constructor (setPolyphony: lastFreeVoiceFound_ = 0), counters kept;
+// one launch on the bank's stream
+extern "C" int mlb_routers_clear(mlb_routers* r)
+{
+  if (!r) return fail(MLB_ERR_INVALID, "null router bank");
+  const size_t words = (size_t)r->G * kRouterWords * 32;
+  const int grid = (int)std::min<size_t>((words + 255) / 256, (size_t)g_sm_count * 8);
+  router_clear_kernel<<<grid, 256, 0, r->stream.get()>>>(r->d_state.get(), words);
+  ++g_launches;
+  CU_CHECK(cudaGetLastError());
+  CU_CHECK(cudaStreamSynchronize(r->stream.get()));
+  return MLB_OK;
+}
+
+extern "C" int mlb_routers_create(int n_instruments, int protocol, const int32_t* polyphony, const int32_t* first_voice,
+                                  const int32_t* unison, const int32_t* mod_cc, int n_voices, mlb_routers** out)
+{
+  if (!out) return fail(MLB_ERR_INVALID, "out is null");
+  *out = nullptr;
+  if (n_instruments <= 0) return fail(MLB_ERR_INVALID, "n_instruments must be positive (got %d)", n_instruments);
+  if (n_voices <= 0) return fail(MLB_ERR_INVALID, "n_voices must be positive (got %d)", n_voices);
+  if (protocol != 0 && protocol != 1) return fail(MLB_ERR_INVALID, "protocol must be 0 (MIDI) or 1 (MPE), got %d", protocol);
+  if (!polyphony || !first_voice) return fail(MLB_ERR_INVALID, "null polyphony or first-voice table");
+  const int G = n_instruments;
+  std::vector<int32_t> inst((size_t)RI_COUNT * G);
+  std::vector<int> owner((size_t)n_voices, -1);
+  for (int g = 0; g < G; ++g)
+  {
+    const int P = polyphony[g];
+    if (P < 0 || P > kRouterVoices - 1)
+      return fail(MLB_ERR_INVALID, "instrument %d: polyphony %d is not in 0..%d", g, P, kRouterVoices - 1);
+    if (unison && unison[g] != 0 && unison[g] != 1)
+      return fail(MLB_ERR_INVALID, "instrument %d: unison %d is not 0 or 1", g, unison[g]);
+    if (mod_cc && (mod_cc[g] < 0 || mod_cc[g] > 128))
+      return fail(MLB_ERR_INVALID, "instrument %d: mod CC %d is not in 0..128", g, mod_cc[g]);
+    const int n = protocol == 1 ? P + 1 : P;
+    if (first_voice[g] < 0 || (int64_t)first_voice[g] + n > n_voices)
+      return fail(MLB_ERR_INVALID, "instrument %d: voices [%d, %lld) are not within the %d voices", g, first_voice[g],
+                  (long long)first_voice[g] + n, n_voices);
+    for (int v = first_voice[g]; v < first_voice[g] + n; ++v)
+    {
+      if (owner[v] >= 0)
+        return fail(MLB_ERR_INVALID, "instrument %d: voice %d belongs to instrument %d already", g, v, owner[v]);
+      owner[v] = g;
+    }
+    inst[(size_t)RI_POLY * G + g] = P;
+    inst[(size_t)RI_FIRST * G + g] = first_voice[g];
+    inst[(size_t)RI_UNISON * G + g] = unison ? unison[g] : 0;
+    inst[(size_t)RI_MOD_CC * G + g] = mod_cc ? mod_cc[g] : 16;  // EventsToSignals::voiceModCC_
+  }
+  std::vector<int32_t> unowned;
+  for (int v = 0; v < n_voices; ++v)
+    if (owner[v] < 0) unowned.push_back(v);
+  MLB_TRY(ensure_init());
+  std::unique_ptr<mlb_routers> r(new mlb_routers);
+  r->live.arm();
+  r->G = G, r->V = n_voices, r->protocol = protocol, r->n_unowned = (int)unowned.size();
+  MLB_TRY(r->d_inst.alloc(inst.size() * 4, "router settings"));
+  MLB_TRY(r->d_state.alloc((size_t)G * kRouterWords * 32 * 4, "router bank"));
+  CU_CHECK(cudaMemcpy(r->d_inst.get(), inst.data(), inst.size() * 4, cudaMemcpyHostToDevice));
+  CU_CHECK(cudaMemset(r->d_state.get(), 0, r->d_state.bytes()));
+  if (!unowned.empty())
+  {
+    MLB_TRY(r->d_unowned.alloc(unowned.size() * 4, "router voice table"));
+    CU_CHECK(cudaMemcpy(r->d_unowned.get(), unowned.data(), unowned.size() * 4, cudaMemcpyHostToDevice));
+  }
+  MLB_TRY(r->stream.create(cudaStreamNonBlocking));
+  *out = r.release();
+  return MLB_OK;
+}
+
+extern "C" int mlb_routers_counters(mlb_routers* r, int64_t* overflow, int64_t* unsupported)
+{
+  if (!r) return fail(MLB_ERR_INVALID, "null router bank");
+  static_assert(RW_SCALAR == RW_OVERFLOW + 1, "the counter words are adjacent");
+  // only the two counter words of each instrument come down, on the bank's stream
+  std::vector<uint32_t> w((size_t)r->G * 64);
+  CU_CHECK(cudaMemcpy2DAsync(w.data(), 64 * 4, r->d_state.get() + RW_OVERFLOW * 32, kRouterWords * 32 * 4, 64 * 4,
+                             r->G, cudaMemcpyDeviceToHost, r->stream.get()));
+  CU_CHECK(cudaStreamSynchronize(r->stream.get()));
+  for (size_t g = 0; g < (size_t)r->G; ++g)
+  {
+    int64_t n = 0;
+    for (int l = 0; l < kRouterVoices; ++l) n += w[g * 64 + l];
+    if (overflow) overflow[g] = n;
+    if (unsupported) unsupported[g] = w[g * 64 + 32 + RS_UNSUPPORTED];
+  }
+  return MLB_OK;
+}
+
+extern "C" int mlb_routers_process_device(mlb_routers* r, const int32_t* offsets_dev, const mlb_event* events_dev,
+                                          mlb_voice_events* records_dev, int32_t* change_offsets_dev,
+                                          mlb_controller_change* changes_dev, int n_blocks, void* stream)
+{
+  if (!r || !offsets_dev || !events_dev || !records_dev || !change_offsets_dev || !changes_dev)
+    return fail(MLB_ERR_INVALID, "null argument");
+  if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive (got %d)", n_blocks);
+  RouterArgs a;
+  a.offsets = offsets_dev, a.events = events_dev, a.records = records_dev;
+  a.change_offsets = change_offsets_dev, a.changes = changes_dev;
+  a.state = r->d_state.get(), a.inst = r->d_inst.get(), a.unowned = r->d_unowned.get();
+  a.n_unowned = r->n_unowned, a.G = r->G, a.V = r->V, a.T = n_blocks, a.mpe = r->protocol;
+  const cudaStream_t s = (cudaStream_t)stream;
+  router_count_kernel<<<n_blocks, kRouterScanThreads, 0, s>>>(a);
+  router_bank_kernel<<<(r->G + kRouterWarps - 1) / kRouterWarps, 32 * kRouterWarps, 0, s>>>(a);
+  router_total_kernel<<<1, kRouterScanThreads, 0, s>>>(change_offsets_dev, r->G, n_blocks);
+  g_launches += 3;
+  CU_CHECK(cudaGetLastError());
+  return MLB_OK;
+}
+
+// offsets [T][G + 1] must index events of n_events entries, non-decreasing within each block, and the referenced events
+// must lie in their vector (time 0..63).  *n_changes = the controller writes they make.
+static int routers_check(const mlb_routers* r, const int32_t* offsets, const mlb_event* events, int n_events,
+                         int n_blocks, int* n_changes)
+{
+  if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive (got %d)", n_blocks);
+  if (n_events < 0) return fail(MLB_ERR_INVALID, "n_events must not be negative (got %d)", n_events);
+  if (n_events > 0 && !events) return fail(MLB_ERR_INVALID, "null events");
+  int64_t n = 0;
+  for (int t = 0; t < n_blocks; ++t)
+  {
+    const int32_t* o = offsets + (size_t)t * (r->G + 1);
+    for (int g = 0; g < r->G; ++g)
+    {
+      if (o[g] < 0 || o[g] > o[g + 1] || o[g + 1] > n_events)
+        return fail(MLB_ERR_INVALID, "block %d, instrument %d: event range [%d, %d) is not within the %d events", t, g,
+                    o[g], o[g + 1], n_events);
+      for (int i = o[g]; i < o[g + 1]; ++i)
+      {
+        if (events[i].time < 0 || events[i].time >= MLB_BLOCK)
+          return fail(MLB_ERR_INVALID, "block %d, instrument %d, event %d: time %d is not a frame of the vector (0..%d)",
+                      t, g, i, (int)events[i].time, MLB_BLOCK - 1);
+        n += router_writes_controller(events[i].type, r->protocol);
+      }
+    }
+  }
+  if (n > 0x7FFFFFFF) return fail(MLB_ERR_INVALID, "%lld controller writes exceed one call", (long long)n);
+  *n_changes = (int)n;
+  return MLB_OK;
+}
+
+extern "C" int mlb_routers_count_changes(mlb_routers* r, const int32_t* offsets_host, const mlb_event* events_host,
+                                         int n_events, int n_blocks, int* n_changes_out)
+{
+  if (!r || !offsets_host || !n_changes_out) return fail(MLB_ERR_INVALID, "null argument");
+  return routers_check(r, offsets_host, events_host, n_events, n_blocks, n_changes_out);
+}
+
+extern "C" int mlb_routers_process_host(mlb_routers* r, const int32_t* offsets_host, const mlb_event* events_host,
+                                        int n_events, mlb_voice_events* records_host, int32_t* change_offsets_host,
+                                        mlb_controller_change* changes_host, int changes_capacity, int* n_changes_out,
+                                        int n_blocks)
+{
+  if (!r || !offsets_host || !records_host || !change_offsets_host) return fail(MLB_ERR_INVALID, "null argument");
+  int n_changes = 0;
+  MLB_TRY(routers_check(r, offsets_host, events_host, n_events, n_blocks, &n_changes));
+  if (n_changes > 0 && !changes_host) return fail(MLB_ERR_INVALID, "null changes (the events make %d writes)", n_changes);
+  if (n_changes > changes_capacity)
+    return fail(MLB_ERR_INVALID, "the events make %d controller writes, changes has room for %d", n_changes,
+                changes_capacity);
+  const size_t T = (size_t)n_blocks, G1 = (size_t)r->G + 1;
+  MLB_TRY(r->d_off.ensure(T * G1 * 4, "staging"));
+  MLB_TRY(r->d_coff.ensure(T * G1 * 4, "staging"));
+  MLB_TRY(r->d_ev.ensure(std::max(n_events, 1) * sizeof(mlb_event), "staging"));
+  MLB_TRY(r->d_rec.ensure(T * r->V * sizeof(mlb_voice_events), "staging"));
+  MLB_TRY(r->d_ch.ensure(std::max(n_changes, 1) * sizeof(mlb_controller_change), "staging"));
+  cudaStream_t s = r->stream.get();
+  const int rc = [&]() -> int
+  {
+    CU_CHECK(cudaMemcpyAsync(r->d_off.get(), offsets_host, T * G1 * 4, cudaMemcpyHostToDevice, s));
+    if (n_events) CU_CHECK(cudaMemcpyAsync(r->d_ev.get(), events_host, n_events * sizeof(mlb_event), cudaMemcpyHostToDevice, s));
+    MLB_TRY(mlb_routers_process_device(r, r->d_off.get(), r->d_ev.get(), r->d_rec.get(), r->d_coff.get(), r->d_ch.get(),
+                                       n_blocks, s));
+    CU_CHECK(cudaMemcpyAsync(records_host, r->d_rec.get(), T * r->V * sizeof(mlb_voice_events), cudaMemcpyDeviceToHost, s));
+    CU_CHECK(cudaMemcpyAsync(change_offsets_host, r->d_coff.get(), T * G1 * 4, cudaMemcpyDeviceToHost, s));
+    if (n_changes)
+      CU_CHECK(cudaMemcpyAsync(changes_host, r->d_ch.get(), n_changes * sizeof(mlb_controller_change),
+                               cudaMemcpyDeviceToHost, s));
+    return MLB_OK;
+  }();
+  if (n_changes_out) *n_changes_out = n_changes;
+  return drain(rc, {s});
+}
+
+// Contract E from raw events: per time chunk on host_pipeline, the chunk's offsets go up on s_h2d (all events with the
+// first chunk); K12, the voice kernel, K11 (if given), the graph and the bus sum (if given) run on the graph's stream
+// into one chunk of device buffers; output or bus rows come down on s_d2h.
+extern "C" int mlb_synth_process_routed_host(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb, mlb_graph* g,
+                                             mlb_buses* b, const int32_t* offsets_host, const mlb_event* events_host,
+                                             int n_events, float* out_host, float* mix_host, float* bus_host,
+                                             int n_blocks)
+{
+  if (!r || !offsets_host) return fail(MLB_ERR_INVALID, "null argument");
+  if (b ? (!bus_host || out_host || mix_host) : bus_host != nullptr)
+    return fail(MLB_ERR_INVALID, "bus rows come with a bus layout, and then alone (out and mix must be null)");
+  const int n_planes = MLB_VOICE_ROWS + (cb ? cb->C : 0);
+  unsigned row_mask;
+  MLB_TRY(synth_check(vb, g, offsets_host, n_blocks, out_host || mix_host || bus_host, &row_mask, n_planes));
+  if (r->V != g->V) return fail(MLB_ERR_INVALID, "router bank writes %d voices, graph has %d", r->V, g->V);
+  if ((r->protocol == 0) != ((vb->flags & MLB_VOICES_MIDI) != 0))
+    return fail(MLB_ERR_INVALID, "router bank protocol %s, voice bank %s MLB_VOICES_MIDI", r->protocol ? "MPE" : "MIDI",
+                (vb->flags & MLB_VOICES_MIDI) ? "with" : "without");
+  if (cb && cb->protocol != r->protocol)
+    return fail(MLB_ERR_INVALID, "router bank protocol %s, controller bank %s", r->protocol ? "MPE" : "MIDI",
+                cb->protocol ? "MPE" : "MIDI");
+  if (cb && cb->G != r->G)
+    return fail(MLB_ERR_INVALID, "router bank has %d instruments, controller bank %d", r->G, cb->G);
+  if (cb && cb->V != g->V)
+    return fail(MLB_ERR_INVALID, "controller bank's voice map has %d voices, graph has %d (mlb_controllers_set_voice_map)",
+                cb->V, g->V);
+  if (b && b->V != g->V) return fail(MLB_ERR_INVALID, "buses are laid over %d voices, graph has %d", b->V, g->V);
+  int n_changes = 0;
+  MLB_TRY(routers_check(r, offsets_host, events_host, n_events, n_blocks, &n_changes));
+  MLB_TRY(ensure_init());
+  const size_t V = (size_t)g->V, T = (size_t)n_blocks, n_out = g->outs.size(), G1 = (size_t)r->G + 1;
+  const int Tc = synth_chunk_blocks(g, n_blocks, n_planes);
+  if (out_host) MLB_TRY(g->d_out.ensure(T * n_out * V * MLB_BLOCK * 4, "staging"));
+  if (b) MLB_TRY(g->d_out.ensure((size_t)Tc * n_out * V * MLB_BLOCK * 4, "staging"));
+  if (b) MLB_TRY(b->d_out.ensure(T * n_out * b->G * MLB_BLOCK * 4, "staging"));
+  if (mix_host) MLB_TRY(g->d_mix.ensure(T * n_out * MLB_BLOCK * 4, "staging"));
+  MLB_TRY(r->d_off.ensure(T * G1 * 4, "staging"));
+  MLB_TRY(r->d_coff.ensure((size_t)Tc * G1 * 4, "staging"));
+  MLB_TRY(r->d_ev.ensure(std::max(n_events, 1) * sizeof(mlb_event), "staging"));
+  MLB_TRY(r->d_ch.ensure(std::max(n_changes, 1) * sizeof(mlb_controller_change), "staging"));
+  MLB_TRY(vb->d_ev.ensure((size_t)Tc * V * sizeof(mlb_voice_events), "staging"));
+  MLB_TRY(vb->d_out.ensure((size_t)Tc * n_planes * V * MLB_BLOCK * 4, "staging"));
+  const size_t row_floats = n_out * V * MLB_BLOCK;             // output rows per block
+  const size_t bus_floats = b ? n_out * b->G * MLB_BLOCK : 0;  // bus rows per block
+  float* down_dev = b ? b->d_out.get() : g->d_out.get();
+  float* down_host = b ? bus_host : out_host;
+  const size_t down_floats = b ? bus_floats : row_floats;
+  const int rc = [&]() -> int
+  {
+    MLB_TRY(host_pipeline(
+        g, n_blocks, Tc, true, down_host != nullptr,
+        [&](int t0, int t1, cudaStream_t s)
+        {
+          cudaError_t e = cudaSuccess;
+          if (t0 == 0 && n_events)
+            e = cudaMemcpyAsync(r->d_ev.get(), events_host, n_events * sizeof(mlb_event), cudaMemcpyHostToDevice, s);
+          if (e == cudaSuccess)
+            e = cudaMemcpyAsync(r->d_off.get() + t0 * G1, offsets_host + t0 * G1, (t1 - t0) * G1 * 4,
+                                cudaMemcpyHostToDevice, s);
+          return e;
+        },
+        [&](int t0, int t1, cudaStream_t s) -> int
+        {
+          MLB_TRY(mlb_routers_process_device(r, r->d_off.get() + t0 * G1, r->d_ev.get(), vb->d_ev.get(), r->d_coff.get(),
+                                             r->d_ch.get(), t1 - t0, s));
+          MLB_TRY(voices_launch(vb, vb->d_ev.get(), vb->d_out.get(), t1 - t0, row_mask, n_planes, s));
+          if (cb)
+            MLB_TRY(mlb_controllers_process_device(cb, r->d_coff.get(), r->d_ch.get(), vb->d_out.get(), MLB_VOICE_ROWS,
+                                                   n_planes, t1 - t0, s));
+          if (b)
+          {
+            MLB_TRY(graph_process(g, vb->d_out.get(), n_planes, g->d_out.get(), nullptr, t1 - t0, s));
+            return mlb_buses_sum_device(b, g->d_out.get(), b->d_out.get() + t0 * bus_floats, (int)n_out, t1 - t0, s);
+          }
+          return graph_process(g, vb->d_out.get(), n_planes, out_host ? g->d_out.get() + t0 * row_floats : nullptr,
+                               mix_host ? g->d_mix.get() + t0 * n_out * MLB_BLOCK : nullptr, t1 - t0, s);
+        },
+        [&](int t0, int t1, cudaStream_t s)
+        {
+          return cudaMemcpyAsync(down_host + t0 * down_floats, down_dev + t0 * down_floats,
+                                 (t1 - t0) * down_floats * 4, cudaMemcpyDeviceToHost, s);
         }));
     if (mix_host) MLB_TRY(mlb_graph_mix_wait(g, g->stream.get()));
     if (mix_host)

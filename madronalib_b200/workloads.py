@@ -902,3 +902,95 @@ def fdtd_inputs(n_instances: int, n_blocks: int, t0: int = 0, v0: int = 0, v1: O
         tri = np.float32(1.0) - np.abs(np.float32(2.0) * ph - np.float32(1.0))
         out[t, 1] = base * (np.float32(1.0) + np.float32(0.1) * tri)
     return out
+
+
+# ---- raw MIDI / MPE events of many instruments, for api.RouterBank (K12) ----
+
+def midi_layout(n_instruments: int, polyphony, mpe: bool = False, gap: int = 0):
+    """Voice layout of G instruments side by side (instrument g's records at voices first_voice[g] ..), with `gap`
+    voices of no instrument after each one.  polyphony: one int or [G].  Returns a dict: polyphony, first_voice [G],
+    n_voices; per voice voice_index (Voice::voiceIndex: MIDI 1..P, MPE 0 = the main voice), main_voice (MPE: the bank
+    index of the voice's main voice or -1; None in MIDI), voice_instrument (-1 for voices of no instrument); and the
+    bus layout bus_first, bus_count of api.Buses (instrument_buses' rule: MPE skips the main voice)."""
+    G = int(n_instruments)
+    poly = np.broadcast_to(np.asarray(polyphony, np.int32), (G,)).copy()
+    n_rec = poly + (1 if mpe else 0)
+    first = np.zeros(G, np.int32)
+    first[1:] = np.cumsum(n_rec + gap)[:-1]
+    V = int(first[-1] + n_rec[-1] + gap) if G else 0
+    vi = np.zeros(V, np.int32)
+    main = np.full(V, -1, np.int32)
+    inst = np.full(V, -1, np.int32)
+    for g in range(G):
+        f, n = int(first[g]), int(n_rec[g])
+        vi[f:f + n] = np.arange(n) + (0 if mpe else 1)
+        inst[f:f + n] = g
+        if mpe:
+            main[f + 1:f + n] = f
+    return dict(polyphony=poly, first_voice=first, n_voices=V, voice_index=vi, main_voice=main if mpe else None,
+                voice_instrument=inst, bus_first=(first + (1 if mpe else 0)).astype(np.int32), bus_count=poly.copy())
+
+
+def midi_performance(n_instruments: int, n_blocks: int, polyphony=8, mpe: bool = False, density: float = 0.1,
+                     seed: int = 21):
+    """A seeded performance of G instruments as raw events: (offsets [T][G + 1] int32, events of api.EVENT_DTYPE),
+    each (block, instrument) range in arrival order with times in 0..63.  In a fraction `density` of the pairs an
+    instrument receives a burst of 1 to 6 events: note-ons (more keys held than voices: stealing), note-offs of held
+    keys, the sustain pedal, pitch bend, note and channel pressure, and CC 1 / 73 / 74 / 123 -- arriving out of time
+    order and now and then at equal times and types.  MPE instruments play on channels 2..16, with bend and pressure
+    on channel 1 as well."""
+    from .api import EVENT_DTYPE
+    rng = np.random.default_rng(seed)
+    G, T = int(n_instruments), int(n_blocks)
+    poly = np.broadcast_to(np.asarray(polyphony, np.int32), (G,))
+    n = np.where(rng.random((T, G)) < density, rng.integers(1, 7, (T, G)), 0)
+    offsets = np.zeros((T, G + 1), np.int32)
+    ends = np.cumsum(n.ravel()).reshape(T, G)
+    offsets[:, 1:] = ends
+    offsets[:, 0] = np.concatenate(([0], ends[:-1, -1])) if T else []
+    total = int(n.sum())
+    ev = np.zeros(total, EVENT_DTYPE)
+    held = [[] for _ in range(G)]
+    pedal = np.zeros(G, bool)
+    # event kinds: 0 note on, 1 note off, 2 pedal, 3 bend, 4 note pressure, 5 channel pressure, 6 CC
+    kinds = rng.choice(7, total, p=[0.34, 0.26, 0.05, 0.1, 0.07, 0.06, 0.12])
+    times = rng.integers(0, 64, total)
+    vals = rng.random((total, 2)).astype(np.float32)
+    i = 0
+    for t in range(T):
+        for g in np.nonzero(n[t])[0]:
+            k0 = i
+            for _ in range(int(n[t, g])):
+                kind, e = int(kinds[i]), ev[i]
+                e["time"] = times[i] if not (i > k0 and rng.random() < 0.25) else ev[i - 1]["time"]
+                e["value1"], e["value2"] = vals[i, 0], np.float32(0.1) + np.float32(0.9) * vals[i, 1]
+                ch = int(rng.integers(2, 17)) if mpe else 1
+                if kind == 1 and held[g]:
+                    key, ch0 = held[g].pop(int(rng.integers(0, len(held[g]))))
+                    e["type"], e["source_idx"], e["channel"] = 4, key, ch0
+                elif kind <= 1:
+                    key = int(rng.integers(36, 97))
+                    if len(held[g]) > 2 * poly[g] + 2:
+                        held[g].pop(0)
+                    held[g].append((key, ch))
+                    e["type"], e["source_idx"], e["channel"] = 1, key, ch
+                    e["value1"] = np.float32(key) / np.float32(12.0)
+                elif kind == 2:
+                    pedal[g] = not pedal[g]
+                    e["type"], e["value1"] = 5, np.float32(1.0 if pedal[g] else 0.0)
+                elif kind == 3:
+                    e["type"], e["channel"] = 7, (1 if mpe and rng.random() < 0.3 else ch)
+                    e["value1"] = np.float32(2.0) * vals[i, 0] - np.float32(1.0)
+                elif kind == 4:
+                    e["type"], e["channel"] = 8, ch
+                    e["source_idx"] = held[g][-1][0] if held[g] else int(rng.integers(36, 97))
+                elif kind == 5:
+                    e["type"], e["channel"] = 9, (1 if mpe and rng.random() < 0.3 else ch)
+                else:
+                    cc = int(rng.choice([1, 1, 73, 74, 74, 123]))
+                    e["type"], e["source_idx"], e["channel"] = 6, cc, ch
+                    if cc == 123:
+                        e["value1"] = np.float32(0.0)
+                        held[g].clear()
+                i += 1
+    return offsets, ev

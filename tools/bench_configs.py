@@ -2,7 +2,7 @@
 """Kernel-resident timing of everything except the headline: BASELINE.json configurations 2-5, the
 SURVEY 8(f) workloads (config 6 = Aaltoverb x V, the EventsToSignals::Voice bank) and the elementwise maps.
 
-    python tools/bench_configs.py [--steps K] [--only 2,3,4,5,6,voices,map,fdtd,buses,controllers] [--generic] [--cpu]
+    python tools/bench_configs.py [--steps K] [--only 2,3,4,5,6,voices,map,fdtd,buses,controllers,router,routed] [--generic] [--cpu]
 
 Prints one JSON line per configuration: kernel name, mean CUDA-event kernel time, algorithmic
 bytes per launch (SURVEY.md 8d / DESIGN.md), achieved GB/s and fraction of the measured HBM peak.
@@ -29,7 +29,7 @@ def main():
     from madronalib_b200 import api, workloads as wl
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
-    ap.add_argument("--only", default="2,3,swept,4,5,6,voices,map,fdtd,buses,controllers")
+    ap.add_argument("--only", default="2,3,swept,4,5,6,voices,map,fdtd,buses,controllers,router,routed")
     ap.add_argument("--generic", action="store_true", help="force the graph interpreter kernel")
     ap.add_argument("--cpu", action="store_true",
                     help="also time the reference (oracle/_ref, all host threads) on config 6, the Voice bank "
@@ -122,6 +122,10 @@ def main():
         bench_buses(api, wl, torch, dev, args.steps)
     if "controllers" in only:
         bench_controllers(api, wl, torch, dev, args.steps)
+    if "router" in only:
+        bench_router(api, wl, torch, dev, args.steps)
+    if "routed" in only:
+        bench_routed(api, wl, torch)
     if args.cpu:
         # the reference itself on this box's host cores (oracle/_ref; checker code, used here only as a baseline)
         import time
@@ -466,6 +470,150 @@ def bench_controllers(api, wl, torch, dev, steps):
           flush=True)
     for h in (g, vb, cb):
         h.close()
+
+
+
+def bench_router(api, wl, torch, dev, steps):
+    """K12 alone, events resident on the device: 4 096 instruments x 16 voices x 64 vectors of midi_performance at
+    its density (0.1) and at 10x, mean of `steps` CUDA-event-timed calls (three launches each) after 2 warm-up calls.
+    Bytes written = the records.  Parity of 16 sampled instruments of a fresh bank's first call against host routers."""
+    import sys
+    sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+    from tests.router_cases import route_on_host
+    G, P, T = 4096, 16, 64
+    facts = gpu_facts()
+    lay = wl.midi_layout(G, P)
+    V = lay["n_voices"]
+    sel = np.linspace(0, G - 1, 16).astype(np.int64)
+    for density in (0.1, 1.0):
+        offsets, ev = wl.midi_performance(G, T, P, density=density, seed=50)
+        d_off = torch.from_numpy(offsets).to(dev)
+        d_ev = torch.from_numpy(ev.view(np.uint8)).to(dev)
+        d_rec = torch.empty((T, V, 72), dtype=torch.uint8, device=dev)
+        d_coff = torch.empty((T, G + 1), dtype=torch.int32, device=dev)
+        d_ch = torch.empty((max(ev.size, 1), 8), dtype=torch.uint8, device=dev)
+        r = api.RouterBank(lay["polyphony"], lay["first_voice"], V)
+        sh = torch.cuda.current_stream().cuda_stream
+        r.process_device(d_off, d_ev, d_rec, d_coff, d_ch, T, stream=sh)
+        torch.cuda.synchronize()
+        got = d_rec.cpu().numpy()
+        for _ in range(2):
+            r.process_device(d_off, d_ev, d_rec, d_coff, d_ch, T, stream=sh)
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(steps):
+            r.process_device(d_off, d_ev, d_rec, d_coff, d_ch, T, stream=sh)
+        e1.record()
+        torch.cuda.synchronize()
+        ms = e0.elapsed_time(e1) / steps
+        r.close()
+        sub_off = np.zeros((T, len(sel) + 1), np.int32)
+        parts, n = [], 0
+        for t in range(T):
+            for j, g in enumerate(sel):
+                sub_off[t, j] = n
+                parts.append(ev[offsets[t, g]:offsets[t, g + 1]])
+                n += parts[-1].size
+            sub_off[t, -1] = n
+        sub_lay = wl.midi_layout(len(sel), P)
+        want = route_on_host(sub_off, np.concatenate(parts), sub_lay)[0]
+        voices = (lay["first_voice"][sel, None] + np.arange(P)[None, :]).reshape(-1)
+        mism = int((got[:, voices].reshape(-1) != np.ascontiguousarray(want).view(np.uint8).reshape(-1)).sum())
+        nbytes = 72.0 * T * V
+        print(json.dumps({
+            "config": "router_%dx%d_density_%g" % (G, P, density), "kernels": "router_count_kernel -> "
+            "router_bank_kernel -> router_total_kernel", "instruments": G, "voices": V, "blocks": T,
+            "events": int(ev.size), "ms_per_call": ms, "record_bytes_written": nbytes,
+            "achieved_gbs": nbytes / (ms * 1e-3) / 1e9,
+            "frac_of_datasheet_hbm": nbytes / (ms * 1e-3) / 1e9 / HBM_DATASHEET_GBS,
+            "datasheet_note": "3.35 TB/s, H100 SXM data sheet", **facts,
+            "parity_instruments": int(len(sel)), "parity_checker": "host routers (mlb::VoiceRouter)",
+            "mismatched_bytes": mism}), flush=True)
+
+
+def host_router_timing(wl, lay, offsets, ev, reps=3):
+    """Compile tools/host_router_timing.cpp into a temporary directory and run it on the performance: one
+    mlb::VoiceRouter per instrument on one host thread.  Returns its JSON line plus the records it produced."""
+    import subprocess
+    import tempfile
+    here = os.path.dirname(os.path.abspath(__file__))
+    G, T = offsets.shape[1] - 1, offsets.shape[0]
+    with tempfile.TemporaryDirectory() as d:
+        exe, inp, out = os.path.join(d, "hrt"), os.path.join(d, "in.bin"), os.path.join(d, "rec.bin")
+        subprocess.run(["g++", "-O2", "-std=c++17", "-I", os.path.join(os.path.dirname(here), "include"),
+                        os.path.join(here, "host_router_timing.cpp"), "-o", exe], check=True)
+        with open(inp, "wb") as f:
+            f.write(np.array([G, T, 0, reps], np.int32).tobytes())
+            f.write(lay["polyphony"].astype(np.int32).tobytes() + lay["first_voice"].astype(np.int32).tobytes())
+            f.write(np.array([lay["n_voices"]], np.int32).tobytes() + offsets.astype(np.int32).tobytes())
+            f.write(np.array([ev.size], np.int32).tobytes() + ev.tobytes())
+        line = json.loads(subprocess.run([exe, inp, out], check=True, capture_output=True, text=True).stdout)
+        line["records"] = np.fromfile(out, wl.VOICE_EVENTS_DTYPE).reshape(T, lay["n_voices"])
+    return line
+
+
+def bench_routed(api, wl, torch, n_calls=5):
+    """Contract E from raw events against contract E from host-routed records, same performance (4 096 instruments x
+    16 voices x 64 vectors of midi_performance, config A, bus rows out), pinned host buffers, host clock around calls
+    that return finished.  The host-routed line adds the wall time of the 4 096 host routers (one thread, this
+    machine's host, timed in C++ by tools/host_router_timing.cpp) that produce its records.  Parity: the two paths' bus rows of the first call, bit for bit."""
+    import ctypes
+    import time
+    from madronalib_b200.api import EVENT_DTYPE
+    G, P, T = 4096, 16, 64
+    facts = gpu_facts()
+    lay = wl.midi_layout(G, P)
+    V = lay["n_voices"]
+    w = wl.config_a(V)
+    vi, gs, da, pb = wl.synth_bank_params(V)
+    offsets, ev = wl.midi_performance(G, T, P, density=0.1, seed=51)
+    L = api.lib()
+    rec = torch.empty((T * V * 72,), dtype=torch.uint8).pin_memory().numpy().view(wl.VOICE_EVENTS_DTYPE).reshape(T, V)
+    host = host_router_timing(wl, lay, offsets, ev, reps=3)
+    rec[:] = host.pop("records")
+    h_bus = [torch.empty((T, 1, G, 64), dtype=torch.float32).pin_memory().numpy() for _ in range(2)]
+    ev_pin = torch.empty((max(ev.size, 1) * 16,), dtype=torch.uint8).pin_memory().numpy().view(EVENT_DTYPE)
+    ev_pin[:ev.size] = ev
+    off_pin = torch.empty(offsets.shape, dtype=torch.int32).pin_memory().numpy()
+    off_pin[:] = offsets
+    results = {}
+    for name in ("host_routed", "routed"):
+        vb = api.VoiceBank(48000.0, lay["voice_index"], gs, da, pb, flags=api.VoiceBank.MIDI)
+        g = api.VoiceGraph(w.spec, V)
+        g.set_coefs(w.coef)
+        g.set_state(w.state)
+        b = api.Buses(V, lay["bus_first"], lay["bus_count"])
+        r = api.RouterBank(lay["polyphony"], lay["first_voice"], V)
+        out = h_bus[0 if name == "host_routed" else 1]
+        if name == "host_routed":
+            call = lambda: L.mlb_synth_process_buses_host(vb._h, g._h, b._h, rec.ctypes.data, out.ctypes.data, T)  # noqa
+            up = rec.nbytes
+        else:
+            call = lambda: L.mlb_synth_process_routed_host(r._h, vb._h, None, g._h, b._h, off_pin.ctypes.data,  # noqa
+                                                           ev_pin.ctypes.data, int(ev.size), None, None,
+                                                           out.ctypes.data, T)
+            up = offsets.nbytes + ev.nbytes
+        assert call() == 0, api.lib().mlb_last_error()
+        first = out.copy()
+        t0 = time.perf_counter()
+        for _ in range(n_calls):
+            call()
+        dt = (time.perf_counter() - t0) / n_calls
+        results[name] = first
+        for h in (vb, g, b, r):
+            h.close()
+        line = {"config": "contract_E_%s_buses" % name, "instruments": G, "voices": V, "blocks": T,
+                "events": int(ev.size), "ms_per_call": 1e3 * dt, "calls_per_s": 1.0 / dt,
+                "voice_samples_per_s": V * T * 64 / dt, "h2d_bytes_per_call": int(up), **facts}
+        if name == "host_routed":
+            line["host_routing_ms"] = host["host_routing_ms"]
+            line["host_routing_note"] = "4 096 mlb::VoiceRouter on one host thread, C++ (tools/host_router_timing.cpp), best of 3"
+            line["ms_per_call_with_host_routing"] = 1e3 * dt + host["host_routing_ms"]
+        print(json.dumps(line), flush=True)
+    a, b_ = results["host_routed"], results["routed"]
+    mism = int(((a.view(np.uint32) != b_.view(np.uint32)) & ~(np.isnan(a) & np.isnan(b_))).sum())
+    print(json.dumps({"config": "contract_E_routed_parity", "checker": "contract E fed by the host routers",
+                      "blocks": T, "mismatches": mism}), flush=True)
 
 
 if __name__ == "__main__":
