@@ -744,6 +744,63 @@ int mlb_synth_process_routed_host(mlb_routers* r, mlb_voices* vb, mlb_controller
                                   const int32_t* offsets_host, const mlb_event* events_host, int n_events,
                                   float* out_host, float* mix_host, float* bus_host, int n_blocks);
 
+/* ---- The host-transport beat phase of G instruments (K13) --------------------------------------
+ * Every reference AudioContext owns one ProcessTime (MLAudioContext.h:23-56, .cpp:16-101): a host calls
+ * AudioContext::updateTime(ppqPos, bpm, isPlaying, sampleRate) (= ProcessTime::setTimeAndRate) with the transport of
+ * the coming block, and every processVector writes the 64-sample quarter-note phasor that getBeatPhase() returns.
+ * A process-time bank holds G such clocks.  Input per block t: the transport updates of instrument g are
+ * transports[offsets[t][g] .. offsets[t][g + 1]) (offsets [T][G + 1] int32, the CSR convention of
+ * mlb_controllers_process_*), applied in order before the block's phase row, each exactly as setTimeAndRate (an update
+ * whose ppq_pos or bpm is NaN or infinite is ignored).  Output [T][n_planes][N][64], the phase in plane plane0; N = G
+ * (instrument rows) or, after mlb_process_time_set_voice_map, N = V, every voice getting its instrument's row (+0 for a
+ * voice of no instrument): the layout of a voice graph's INPUT planes.  Bit for bit the reference's rows and state. */
+typedef struct mlb_transport {
+  double ppq_pos;            /* quarter notes since the start of the song, at the start of the block */
+  double bpm;
+  double sample_rate;
+  int32_t is_playing;        /* nonzero: playing */
+  int32_t pad;
+} mlb_transport;             /* 32 bytes */
+typedef struct mlb_process_time mlb_process_time;
+/* State words [MLB_PT_WORDS][G] uint64, ProcessTime's members in this order: omega_ (the float's bits in the low 32
+ * bits), dpdt_, ppqPos1_, ppqPhase1_ (the doubles' bits), playing1_, active1_ (0 / 1), samplesSincePreviousTime_,
+ * samplesSinceStart, bpm, sampleRate (the doubles' bits). */
+#define MLB_PT_WORDS 10
+enum { MLB_PT_OMEGA = 0, MLB_PT_DPDT, MLB_PT_PPQ_POS1, MLB_PT_PPQ_PHASE1, MLB_PT_PLAYING1, MLB_PT_ACTIVE1,
+       MLB_PT_SAMPLES_PREV, MLB_PT_SAMPLES_START, MLB_PT_BPM, MLB_PT_SAMPLE_RATE };
+/* Every clock as AudioContext(nIn, nOut, sample_rate) leaves it: all members at their defaults (ppqPos1_ = -1) and
+ * sampleRate = sample_rate.  That constructor takes an int, so sample_rate must be a whole number of hertz
+ * (1..INT_MAX); MLB_ERR_INVALID for a fractional or out-of-range rate and for n_instruments < 1.  Transport updates
+ * then set sampleRate to their own (double) sample_rate, as updateTime does.  A live bank counts toward mlb_init's
+ * one-device rule. */
+int mlb_process_time_create(int n_instruments, double sample_rate, mlb_process_time** out);
+int mlb_process_time_destroy(mlb_process_time* pt);
+/* ProcessTime::clear() of every clock (.cpp:80-85): dpdt_ = 0, active1_ = playing1_ = false; omega_ and the rest are
+ * kept, as in the reference.  Ordered as mlb_controllers_clear. */
+int mlb_process_time_clear(mlb_process_time* pt);
+int mlb_process_time_get_state(mlb_process_time* pt, uint64_t* words);
+int mlb_process_time_set_state(mlb_process_time* pt, const uint64_t* words);
+/* voice_instrument[V]: the instrument of each voice, or -1; NULL goes back to instrument rows */
+int mlb_process_time_set_voice_map(mlb_process_time* pt, const int32_t* voice_instrument, int n_voices);
+/* one launch for n_blocks vectors, no allocation, no synchronisation (capturable into a CUDA graph) */
+int mlb_process_time_process_device(mlb_process_time* pt, const int32_t* offsets_dev, const mlb_transport* transports_dev,
+                                    float* out_dev, int plane0, int n_planes, int n_blocks, void* stream);
+/* host buffers: offsets are checked (non-decreasing per block, within [0, n_transports]) before anything is copied;
+ * only plane plane0 of out_host is written */
+int mlb_process_time_process_host(mlb_process_time* pt, const int32_t* offsets_host, const mlb_transport* transports_host,
+                                  int n_transports, float* out_host, int plane0, int n_planes, int n_blocks);
+/* Contract E with every AudioContext signal a voice reads: mlb_synth_process_routed_host, plus K13 after the
+ * controller bank in each time chunk.  The graph's input per block is the 8 Voice rows (getInputVoice), then the C
+ * controller planes when a controller bank is given (getInputController), then one beat-phase plane when a
+ * process-time bank is given (getBeatPhase): INPUT plane 8 + C.  time_offsets_host [T][G + 1] into transports_host
+ * (both ignored without a process-time bank); everything else as mlb_synth_process_routed_host.  MLB_ERR_INVALID,
+ * before anything is copied, also names a process-time bank of another instrument count or voice map, bad transport
+ * offsets, and a graph INPUT plane beyond the beat phase. */
+int mlb_synth_process_context_host(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb, mlb_process_time* pt,
+                                   mlb_graph* g, mlb_buses* b, const int32_t* offsets_host, const mlb_event* events_host,
+                                   int n_events, const int32_t* time_offsets_host, const mlb_transport* transports_host,
+                                   int n_transports, float* out_host, float* mix_host, float* bus_host, int n_blocks);
+
 #ifdef __cplusplus
 }
 #endif

@@ -817,6 +817,60 @@ inline void processEventsRouted(RouterBank& routers, VoiceBank& voices, Controll
                                       mix, bus, nBlocks));
 }
 
+// ---- ProcessTimeBank: the host-transport beat phase of G instruments (mlb_process_time_*), what
+// AudioContext::getBeatPhase() returns after AudioContext::updateTime ----
+class ProcessTimeBank
+{
+  mlb_process_time* p_ = nullptr;
+  int instruments_ = 0;
+
+ public:
+  explicit ProcessTimeBank(int nInstruments, double sampleRate = 48000.) : instruments_(nInstruments)
+  {
+    check(mlb_process_time_create(nInstruments, sampleRate, &p_));
+  }
+  ~ProcessTimeBank() { mlb_process_time_destroy(p_); }
+  ProcessTimeBank(const ProcessTimeBank&) = delete;
+  ProcessTimeBank& operator=(const ProcessTimeBank&) = delete;
+  int instruments() const { return instruments_; }
+  mlb_process_time* handle() const { return p_; }
+  // ProcessTime::clear() of every clock (dpdt_, active1_, playing1_ only, as in the reference)
+  void clear() { check(mlb_process_time_clear(p_)); }
+  // words [MLB_PT_WORDS][instruments]
+  void getState(uint64_t* words) { check(mlb_process_time_get_state(p_, words)); }
+  void setState(const uint64_t* words) { check(mlb_process_time_set_state(p_, words)); }
+  // voiceInstrument[nVoices]: each voice's instrument or -1; nullptr goes back to instrument rows
+  void setVoiceMap(const int32_t* voiceInstrument, int nVoices) { check(mlb_process_time_set_voice_map(p_, voiceInstrument, nVoices)); }
+  // host buffers: offsets [nBlocks][instruments + 1] into transports -> plane plane0 of
+  // out [nBlocks][nPlanes][instruments or voices][64]
+  void process(const int32_t* offsets, const mlb_transport* transports, int nTransports, float* out, int plane0,
+               int nPlanes, int nBlocks)
+  {
+    check(mlb_process_time_process_host(p_, offsets, transports, nTransports, out, plane0, nPlanes, nBlocks));
+  }
+  // device buffers, asynchronous on `stream`: one launch, no allocation or synchronisation
+  void processDevice(const int32_t* offsets, const mlb_transport* transports, float* out, int plane0, int nPlanes,
+                     int nBlocks, void* stream = nullptr)
+  {
+    check(mlb_process_time_process_device(p_, offsets, transports, out, plane0, nPlanes, nBlocks, stream));
+  }
+};
+
+// Contract E with every AudioContext signal (mlb_synth_process_context_host): processEventsRouted, plus the beat
+// phase of `times` (if given), fed by timeOffsets [nBlocks][instruments + 1] into transports.  The graph's INPUT
+// planes are the 8 Voice rows, then the controller planes, then the beat phase.
+inline void processEventsWithContext(RouterBank& routers, VoiceBank& voices, ControllerBank* controllers,
+                                     ProcessTimeBank* times, DeviceBank& bank, Buses* buses, const int32_t* offsets,
+                                     const mlb_event* events, int nEvents, const int32_t* timeOffsets,
+                                     const mlb_transport* transports, int nTransports, float* out, float* mix,
+                                     float* bus, int nBlocks)
+{
+  check(mlb_synth_process_context_host(routers.handle(), voices.handle(), controllers ? controllers->handle() : nullptr,
+                                       times ? times->handle() : nullptr, bank.handle(),
+                                       buses ? buses->handle() : nullptr, offsets, events, nEvents, timeOffsets,
+                                       transports, nTransports, out, mix, bus, nBlocks));
+}
+
 // ---- Resampler: Upsampler(octaves) / Downsampler(octaves) x V on the GPU (mlb_resampler_*) ----
 class Resampler
 {

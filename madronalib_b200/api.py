@@ -128,6 +128,17 @@ def lib() -> ctypes.CDLL:
     L.mlb_routers_count_changes.argtypes = [_vp, _vp, _vp, ctypes.c_int, ctypes.c_int, _vp]
     L.mlb_synth_process_routed_host.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int, _vp, _vp, _vp,
                                                 ctypes.c_int]
+    L.mlb_process_time_create.argtypes = [ctypes.c_int, ctypes.c_double, _vp]
+    L.mlb_process_time_destroy.argtypes = [_vp]
+    L.mlb_process_time_clear.argtypes = [_vp]
+    L.mlb_process_time_get_state.argtypes = [_vp, _vp]
+    L.mlb_process_time_set_state.argtypes = [_vp, _vp]
+    L.mlb_process_time_set_voice_map.argtypes = [_vp, _vp, ctypes.c_int]
+    L.mlb_process_time_process_device.argtypes = [_vp, _vp, _vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
+    L.mlb_process_time_process_host.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp, ctypes.c_int, ctypes.c_int,
+                                                ctypes.c_int]
+    L.mlb_synth_process_context_host.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int, _vp, _vp,
+                                                 ctypes.c_int, _vp, _vp, _vp, ctypes.c_int]
     L.mlb_graph_process_host.argtypes = [_vp, _vp, _vp, _vp, ctypes.c_int]
     L.mlb_graph_last_kernel_ms.argtypes = [_vp, _vp]
     L.mlb_graph_last_host_slices.argtypes = [_vp]
@@ -200,8 +211,8 @@ def kernel_launches() -> int:
 
 
 def live_handles() -> int:
-    """Graphs, voice banks, bus layouts, controller banks, resamplers, FDTD banks and mix buses alive in this
-    process."""
+    """Graphs, voice banks, bus layouts, controller banks, process-time banks, router banks, resamplers, FDTD banks
+    and mix buses alive in this process."""
     return int(lib().mlb_live_handles())
 
 
@@ -487,6 +498,41 @@ class VoiceGraph(_Handle):
                                                    _ptr(mix), _ptr(bus), T))
         return bus if buses is not None else (out, mix)
 
+    def process_context_host(self, routers: "RouterBank", bank: "VoiceBank", offsets: np.ndarray, events: np.ndarray,
+                             controllers: Optional["ControllerBank"] = None, times: Optional["ProcessTimeBank"] = None,
+                             time_offsets: Optional[np.ndarray] = None, transports: Optional[np.ndarray] = None,
+                             buses: Optional["Buses"] = None, want_out: bool = True, want_mix: bool = False):
+        """Contract E with every AudioContext signal (mlb_synth_process_context_host): process_routed_host, plus the
+        beat phase of ``times`` (if given) fed by time_offsets [T][G + 1] into transports (TRANSPORT_DTYPE).  The
+        graph's INPUT planes are the 8 Voice rows, then the controller planes, then the beat phase.  Returns as
+        process_routed_host."""
+        s, V = self.spec, self.n_voices
+        off = np.ascontiguousarray(offsets, np.int32)
+        if off.ndim != 2 or off.shape[1] != routers.n_instruments + 1:
+            raise ValueError(f"process_context_host: offsets must be [T][{routers.n_instruments + 1}], got {off.shape}")
+        ev = np.ascontiguousarray(events, EVENT_DTYPE)
+        T = int(off.shape[0])
+        toff = tr = None
+        if times is not None:
+            if time_offsets is None or transports is None:
+                raise ValueError("process_context_host: a process-time bank needs time_offsets and transports")
+            toff = np.ascontiguousarray(time_offsets, np.int32)
+            if toff.shape != off.shape:
+                raise ValueError(f"process_context_host: time_offsets must be {off.shape}, got {toff.shape}")
+            tr = np.ascontiguousarray(transports, TRANSPORT_DTYPE)
+        out = mix = bus = None
+        if buses is not None:
+            bus = np.empty((T, s.n_out, buses.n_buses, BLOCK), np.float32)
+        else:
+            out = np.empty((T, s.n_out, V, BLOCK), np.float32) if want_out else None
+            mix = np.empty((T, s.n_out, BLOCK), np.float32) if want_mix else None
+        _check(lib().mlb_synth_process_context_host(
+            routers._h, bank._h, controllers._h if controllers else None, times._h if times else None, self._h,
+            buses._h if buses else None, off.ctypes.data, ev.ctypes.data if ev.size else None, int(ev.size),
+            _ptr(toff), tr.ctypes.data if tr is not None and tr.size else None, 0 if tr is None else int(tr.size),
+            _ptr(out), _ptr(mix), _ptr(bus), T))
+        return bus if buses is not None else (out, mix)
+
     def process_device(self, inp, out, mix, n_blocks: int, stream: int = 0) -> None:
         """Device pointers (torch tensors / ints); asynchronous on ``stream`` (cudaStream_t)."""
         _check(lib().mlb_graph_process_device(self._h, _ptr(inp), _ptr(out), _ptr(mix), int(n_blocks),
@@ -703,6 +749,82 @@ class ControllerBank(_Handle):
         P = self.n_controllers if n_planes is None else int(n_planes)
         _check(lib().mlb_controllers_process_device(self._h, _ptr(offsets), _ptr(changes), _ptr(out), int(plane0), P,
                                                     int(n_blocks), stream or None))
+
+
+TRANSPORT_DTYPE = np.dtype([("ppq_pos", "<f8"), ("bpm", "<f8"), ("sample_rate", "<f8"), ("is_playing", "<i4"),
+                            ("pad", "<i4")])  # mlb_transport
+
+
+class ProcessTimeBank(_Handle):
+    """G host-transport clocks (mlb_process_time_*): the AudioContext::ProcessTime of one reference AudioContext per
+    instrument, i.e. what AudioContext::getBeatPhase() returns, bit for bit.  Input per block: a CSR list of transport
+    updates, offsets [T][G + 1] into transports (TRANSPORT_DTYPE), each applied in order as
+    AudioContext::updateTime before the block; output [T][n_planes][N][64] with the phase in plane plane0 and N = G,
+    or N = V after set_voice_map (every voice gets its instrument's row, a voice of instrument -1 gets +0)."""
+
+    _destroy = "mlb_process_time_destroy"
+
+    N_WORDS = 10  # omega_, dpdt_, ppqPos1_, ppqPhase1_, playing1_, active1_, samplesSincePreviousTime_,
+    #               samplesSinceStart, bpm, sampleRate
+
+    def __init__(self, n_instruments: int, sample_rate: float = 48000.0):
+        """sample_rate: whole hertz, as AudioContext(nIn, nOut, int rate) takes it (a fractional rate is refused)."""
+        self.n_instruments, self.n_voices = int(n_instruments), 0
+        h = ctypes.c_void_p()
+        _check(lib().mlb_process_time_create(self.n_instruments, float(sample_rate), ctypes.byref(h)))
+        self._h = h
+
+    def clear(self) -> None:
+        """ProcessTime::clear() of every clock: dpdt_, active1_ and playing1_ only."""
+        _check(lib().mlb_process_time_clear(self._h))
+
+    def get_state(self) -> np.ndarray:
+        """words [10][G] uint64: a float's bits in the low 32 bits, a double's bits, a bool as 0 / 1, a counter."""
+        w = np.zeros((self.N_WORDS, self.n_instruments), np.uint64)
+        _check(lib().mlb_process_time_get_state(self._h, w.ctypes.data))
+        return w
+
+    def set_state(self, words: np.ndarray) -> None:
+        w = np.ascontiguousarray(words, np.uint64)
+        if w.shape != (self.N_WORDS, self.n_instruments):
+            raise ValueError(f"set_state: words must be [10][{self.n_instruments}], got {w.shape}")
+        _check(lib().mlb_process_time_set_state(self._h, w.ctypes.data))
+
+    def set_voice_map(self, voice_instrument) -> None:
+        """voice_instrument[V]: each voice's instrument or -1; None goes back to instrument rows."""
+        if voice_instrument is None:
+            _check(lib().mlb_process_time_set_voice_map(self._h, None, 0))
+            self.n_voices = 0
+            return
+        vm = np.ascontiguousarray(voice_instrument, np.int32)
+        _check(lib().mlb_process_time_set_voice_map(self._h, vm.ctypes.data, int(vm.shape[0])))
+        self.n_voices = int(vm.shape[0])
+
+    def process_host(self, offsets: np.ndarray, transports: np.ndarray, out: Optional[np.ndarray] = None,
+                     plane0: int = 0, n_planes: int = 1) -> np.ndarray:
+        """offsets [T][G + 1] int32, transports (TRANSPORT_DTYPE) -> out [T][n_planes][N][64]; planes other than
+        plane0 of a given `out` are left as they are."""
+        off = np.ascontiguousarray(offsets, np.int32)
+        if off.ndim != 2 or off.shape[1] != self.n_instruments + 1:
+            raise ValueError(f"process_host: offsets must be [T][{self.n_instruments + 1}], got {off.shape}")
+        tr = np.ascontiguousarray(transports, TRANSPORT_DTYPE)
+        T = int(off.shape[0])
+        shape = (T, int(n_planes), self.n_voices or self.n_instruments, BLOCK)
+        if out is None:
+            out = np.zeros(shape, np.float32)
+        if not (isinstance(out, np.ndarray) and out.dtype == np.float32 and out.flags["C_CONTIGUOUS"] and
+                out.shape == shape):
+            raise ValueError(f"process_host: `out` must be a C-contiguous float32 array of shape {shape}")
+        _check(lib().mlb_process_time_process_host(self._h, off.ctypes.data, tr.ctypes.data if tr.size else None,
+                                                   int(tr.size), out.ctypes.data, int(plane0), int(n_planes), T))
+        return out
+
+    def process_device(self, offsets, transports, out, n_blocks: int, plane0: int = 0, n_planes: int = 1,
+                       stream: int = 0) -> None:
+        """Device buffers (torch tensors / ints); asynchronous on ``stream``, one kernel launch, no allocation or
+        synchronisation (capturable into a CUDA graph)."""
+        _check(lib().mlb_process_time_process_device(self._h, _ptr(offsets), _ptr(transports), _ptr(out), int(plane0),
+                                                     int(n_planes), int(n_blocks), stream or None))
 
 
 class ResamplerBank(_Handle):

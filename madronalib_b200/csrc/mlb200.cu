@@ -31,6 +31,7 @@
 #include "bus_kernel.cuh"
 #include "controller_kernel.cuh"
 #include "router_kernel.cuh"
+#include "process_time_kernel.cuh"
 #include "generic_kernel.cuh"
 
 using namespace mlb;
@@ -2533,7 +2534,7 @@ extern "C" int mlb_voices_process_host(mlb_voices* vb, const mlb_voice_events* e
 // n_planes: the input planes per block, the 8 Voice rows and any controller planes after them.
 // events_host: the records, or the raw events' offsets of the routed entry point.
 static int synth_check(const mlb_voices* vb, const mlb_graph* g, const void* events_host, int n_blocks,
-                       bool wants_output, unsigned* row_mask, int n_planes = MLB_VOICE_ROWS)
+                       bool wants_output, unsigned* row_mask, int n_planes = MLB_VOICE_ROWS, bool phase_plane = false)
 {
   if (!vb || !g || !events_host) return fail(MLB_ERR_INVALID, "null argument");
   MLB_TRY(graph_check(g, n_blocks, n_planes, events_host, wants_output));
@@ -2544,7 +2545,10 @@ static int synth_check(const mlb_voices* vb, const mlb_graph* g, const void* eve
     if (n.op == MLB_OP_INPUT)
     {
       if (n.iarg < 0 || n.iarg >= n_planes)
-        return n_planes == MLB_VOICE_ROWS
+        return phase_plane
+                   ? fail(MLB_ERR_INVALID, "graph INPUT plane %d is not a Voice row, controller plane or the beat-phase "
+                          "plane (0..%d)", n.iarg, n_planes - 1)
+               : n_planes == MLB_VOICE_ROWS
                    ? fail(MLB_ERR_INVALID, "graph INPUT plane %d is not a Voice row (0..%d)", n.iarg, MLB_VOICE_ROWS - 1)
                    : fail(MLB_ERR_INVALID, "graph INPUT plane %d is not a Voice row or controller plane (0..%d)", n.iarg,
                           n_planes - 1);
@@ -2807,17 +2811,17 @@ extern "C" int mlb_controllers_set_state(mlb_controllers* cb, const uint32_t* wo
   return MLB_OK;
 }
 
-extern "C" int mlb_controllers_set_voice_map(mlb_controllers* cb, const int32_t* voice_instrument, int n_voices)
+// The device voice map of the controller and process-time banks: [G + 2] offsets, then the V voices grouped by
+// instrument, the unmapped (-1) ones last.  Sets *V.
+static int upload_voice_map(int G, const int32_t* voice_instrument, int n_voices, DevBuf<int32_t>& d_vmap, int* V)
 {
-  if (!cb) return fail(MLB_ERR_INVALID, "null controller bank");
   if (!voice_instrument)
   {
-    cb->d_vmap.reset();
-    cb->V = 0;
+    d_vmap.reset();
+    *V = 0;
     return MLB_OK;
   }
   if (n_voices <= 0) return fail(MLB_ERR_INVALID, "n_voices must be positive (got %d)", n_voices);
-  const int G = cb->G;
   std::vector<int32_t> tab((size_t)G + 2 + n_voices, 0);  // counting sort by instrument, the unmapped (-1) ones last
   for (int v = 0; v < n_voices; ++v)
   {
@@ -2833,10 +2837,16 @@ extern "C" int mlb_controllers_set_voice_map(mlb_controllers* cb, const int32_t*
     const int g = voice_instrument[v] < 0 ? G : voice_instrument[v];
     tab[(size_t)G + 2 + fill[g]++] = v;
   }
-  MLB_TRY(cb->d_vmap.alloc(tab.size() * 4, "voice map"));
-  CU_CHECK(cudaMemcpy(cb->d_vmap.get(), tab.data(), tab.size() * 4, cudaMemcpyHostToDevice));
-  cb->V = n_voices;
+  MLB_TRY(d_vmap.alloc(tab.size() * 4, "voice map"));
+  CU_CHECK(cudaMemcpy(d_vmap.get(), tab.data(), tab.size() * 4, cudaMemcpyHostToDevice));
+  *V = n_voices;
   return MLB_OK;
+}
+
+extern "C" int mlb_controllers_set_voice_map(mlb_controllers* cb, const int32_t* voice_instrument, int n_voices)
+{
+  if (!cb) return fail(MLB_ERR_INVALID, "null controller bank");
+  return upload_voice_map(cb->G, voice_instrument, n_voices, cb->d_vmap, &cb->V);
 }
 
 extern "C" int mlb_controllers_process_device(mlb_controllers* cb, const int32_t* offsets_dev,
@@ -2983,6 +2993,157 @@ extern "C" int mlb_synth_process_controllers_host(mlb_voices* vb, mlb_controller
     return MLB_OK;
   }();
   return drain(rc, {g->s_h2d.get(), g->stream.get(), g->s_d2h.get()});
+}
+
+// ------------------------------------------------------------------------------------------
+// The host-transport beat phase of G instruments (K13, process_time_kernel.cuh)
+
+struct mlb_process_time
+{
+  // declared first, so released last: the buffers below are freed first, and cudaFree waits for the device
+  LiveCount live;
+  Stream stream;
+  int G = 0;
+  int V = 0;                 // voices of the voice map; 0: instrument rows
+  DevBuf<uint64_t> d_state;  // [MLB_PT_WORDS][G]
+  DevBuf<int32_t> d_vmap;    // upload_voice_map's table
+  DevBuf<int32_t> d_off;     // staging of the host entry points
+  DevBuf<mlb_transport> d_tr;
+  DevBuf<float> d_out;
+};
+
+extern "C" int mlb_process_time_destroy(mlb_process_time* pt)
+{
+  delete pt;
+  return MLB_OK;
+}
+
+extern "C" int mlb_process_time_create(int n_instruments, double sample_rate, mlb_process_time** out)
+{
+  if (!out) return fail(MLB_ERR_INVALID, "out is null");
+  *out = nullptr;
+  if (n_instruments <= 0) return fail(MLB_ERR_INVALID, "n_instruments must be positive (got %d)", n_instruments);
+  // AudioContext(nIn, nOut, int rate) and setSampleRate(int) take whole hertz: a fractional rate is refused rather
+  // than truncated behind the caller's back
+  if (!(sample_rate >= 1. && sample_rate <= 2147483647.) || sample_rate != std::floor(sample_rate))
+    return fail(MLB_ERR_INVALID, "sample_rate must be a whole number of hertz in 1..2147483647, as "
+                "AudioContext(nIn, nOut, int rate) takes it (got %.17g)", sample_rate);
+  MLB_TRY(ensure_init());
+  std::unique_ptr<mlb_process_time> pt(new mlb_process_time);
+  pt->live.arm();
+  pt->G = n_instruments;
+  const size_t G = (size_t)n_instruments;
+  MLB_TRY(pt->d_state.alloc((size_t)MLB_PT_WORDS * G * 8, "process-time bank"));
+  // ProcessTime's member defaults (MLAudioContext.h:43-56), then AudioContext::setSampleRate
+  std::vector<uint64_t> st((size_t)MLB_PT_WORDS * G, 0u);
+  const double ppq1 = -1.;
+  uint64_t ppq1_bits, sr_bits;
+  memcpy(&ppq1_bits, &ppq1, 8);
+  memcpy(&sr_bits, &sample_rate, 8);
+  std::fill_n(st.begin() + MLB_PT_PPQ_POS1 * G, G, ppq1_bits);
+  std::fill_n(st.begin() + MLB_PT_SAMPLE_RATE * G, G, sr_bits);
+  CU_CHECK(cudaMemcpy(pt->d_state.get(), st.data(), st.size() * 8, cudaMemcpyHostToDevice));
+  MLB_TRY(pt->stream.create(cudaStreamNonBlocking));
+  *out = pt.release();
+  return MLB_OK;
+}
+
+extern "C" int mlb_process_time_clear(mlb_process_time* pt)
+{
+  if (!pt) return fail(MLB_ERR_INVALID, "null process-time bank");
+  const size_t G = (size_t)pt->G;
+  // ProcessTime::clear (.cpp:80-85): dpdt_ = 0. (all-zero bits), active1_ = playing1_ = false
+  for (int w : {(int)MLB_PT_DPDT, (int)MLB_PT_PLAYING1, (int)MLB_PT_ACTIVE1})
+    CU_CHECK(cudaMemset(pt->d_state.get() + w * G, 0, G * 8));
+  return MLB_OK;
+}
+
+extern "C" int mlb_process_time_get_state(mlb_process_time* pt, uint64_t* words)
+{
+  if (!pt || !words) return fail(MLB_ERR_INVALID, "null argument");
+  CU_CHECK(cudaMemcpy(words, pt->d_state.get(), pt->d_state.bytes(), cudaMemcpyDeviceToHost));
+  return MLB_OK;
+}
+
+extern "C" int mlb_process_time_set_state(mlb_process_time* pt, const uint64_t* words)
+{
+  if (!pt || !words) return fail(MLB_ERR_INVALID, "null argument");
+  CU_CHECK(cudaMemcpy(pt->d_state.get(), words, pt->d_state.bytes(), cudaMemcpyHostToDevice));
+  return MLB_OK;
+}
+
+extern "C" int mlb_process_time_set_voice_map(mlb_process_time* pt, const int32_t* voice_instrument, int n_voices)
+{
+  if (!pt) return fail(MLB_ERR_INVALID, "null process-time bank");
+  return upload_voice_map(pt->G, voice_instrument, n_voices, pt->d_vmap, &pt->V);
+}
+
+extern "C" int mlb_process_time_process_device(mlb_process_time* pt, const int32_t* offsets_dev,
+                                               const mlb_transport* transports_dev, float* out_dev, int plane0,
+                                               int n_planes, int n_blocks, void* stream)
+{
+  if (!pt || !offsets_dev || !out_dev) return fail(MLB_ERR_INVALID, "null argument");
+  if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive (got %d)", n_blocks);
+  if (plane0 < 0 || n_planes <= plane0)
+    return fail(MLB_ERR_INVALID, "beat-phase plane %d is not within the %d output planes", plane0, n_planes);
+  PtArgs a;
+  a.offsets = offsets_dev, a.tr = transports_dev, a.state = pt->d_state.get(), a.out = out_dev;
+  a.vmap_off = pt->V ? pt->d_vmap.get() : nullptr;
+  a.vmap_voice = pt->V ? pt->d_vmap.get() + pt->G + 2 : nullptr;
+  a.G = pt->G, a.N = pt->V ? pt->V : pt->G, a.T = n_blocks;
+  a.plane0 = plane0, a.n_planes = n_planes;
+  a.n_gblk = (pt->G + 31) / 32;
+  process_time_kernel<<<(unsigned)((a.n_gblk + kPtWarps - 1) / kPtWarps), 32 * kPtWarps, 0, (cudaStream_t)stream>>>(a);
+  ++g_launches;
+  CU_CHECK(cudaGetLastError());
+  return MLB_OK;
+}
+
+// offsets [T][G + 1] must index transports of n_transports entries, non-decreasing within each block
+static int process_time_check_offsets(const mlb_process_time* pt, const int32_t* offsets, int n_transports, int n_blocks)
+{
+  for (int t = 0; t < n_blocks; ++t)
+  {
+    const int32_t* o = offsets + (size_t)t * (pt->G + 1);
+    for (int g = 0; g < pt->G; ++g)
+      if (o[g] < 0 || o[g] > o[g + 1] || o[g + 1] > n_transports)
+        return fail(MLB_ERR_INVALID, "block %d, instrument %d: transport range [%d, %d) is not within the %d updates", t,
+                    g, o[g], o[g + 1], n_transports);
+  }
+  return MLB_OK;
+}
+
+extern "C" int mlb_process_time_process_host(mlb_process_time* pt, const int32_t* offsets_host,
+                                             const mlb_transport* transports_host, int n_transports, float* out_host,
+                                             int plane0, int n_planes, int n_blocks)
+{
+  if (!pt || !offsets_host || !out_host || (n_transports > 0 && !transports_host))
+    return fail(MLB_ERR_INVALID, "null argument");
+  if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive (got %d)", n_blocks);
+  if (n_transports < 0) return fail(MLB_ERR_INVALID, "n_transports must not be negative (got %d)", n_transports);
+  MLB_TRY(process_time_check_offsets(pt, offsets_host, n_transports, n_blocks));
+  if (plane0 < 0 || n_planes <= plane0)
+    return fail(MLB_ERR_INVALID, "beat-phase plane %d is not within the %d output planes", plane0, n_planes);
+  const size_t T = (size_t)n_blocks, N = pt->V ? pt->V : pt->G;
+  const size_t off_bytes = T * (pt->G + 1) * 4, tr_bytes = (size_t)n_transports * sizeof(mlb_transport);
+  MLB_TRY(pt->d_off.ensure(off_bytes, "staging"));
+  if (n_transports) MLB_TRY(pt->d_tr.ensure(tr_bytes, "staging"));
+  MLB_TRY(pt->d_out.ensure(T * n_planes * N * MLB_BLOCK * 4, "staging"));
+  cudaStream_t s = pt->stream.get();
+  const int rc = [&]() -> int
+  {
+    CU_CHECK(cudaMemcpyAsync(pt->d_off.get(), offsets_host, off_bytes, cudaMemcpyHostToDevice, s));
+    if (n_transports) CU_CHECK(cudaMemcpyAsync(pt->d_tr.get(), transports_host, tr_bytes, cudaMemcpyHostToDevice, s));
+    MLB_TRY(mlb_process_time_process_device(pt, pt->d_off.get(), pt->d_tr.get(), pt->d_out.get(), plane0, n_planes,
+                                            n_blocks, s));
+    // only the phase plane comes down: the caller's other planes stay as they were
+    const size_t plane = N * MLB_BLOCK * 4, pitch = (size_t)n_planes * plane;
+    CU_CHECK(cudaMemcpy2DAsync(reinterpret_cast<char*>(out_host) + plane0 * plane, pitch,
+                               reinterpret_cast<const char*>(pt->d_out.get()) + plane0 * plane, pitch, plane, T,
+                               cudaMemcpyDeviceToHost, s));
+    return MLB_OK;
+  }();
+  return drain(rc, {s});
 }
 
 // ------------------------------------------------------------------------------------------
@@ -3194,20 +3355,22 @@ extern "C" int mlb_routers_process_host(mlb_routers* r, const int32_t* offsets_h
   return drain(rc, {s});
 }
 
-// Contract E from raw events: per time chunk on host_pipeline, the chunk's offsets go up on s_h2d (all events with the
-// first chunk); K12, the voice kernel, K11 (if given), the graph and the bus sum (if given) run on the graph's stream
-// into one chunk of device buffers; output or bus rows come down on s_d2h.
-extern "C" int mlb_synth_process_routed_host(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb, mlb_graph* g,
-                                             mlb_buses* b, const int32_t* offsets_host, const mlb_event* events_host,
-                                             int n_events, float* out_host, float* mix_host, float* bus_host,
-                                             int n_blocks)
+// Contract E from raw events: per time chunk on host_pipeline, the chunk's offsets go up on s_h2d (all events and
+// transport updates with the first chunk); K12, the voice kernel, K11 (if given), K13 (if given), the graph and the bus
+// sum (if given) run on the graph's stream into one chunk of device buffers; output or bus rows come down on s_d2h.
+static int synth_routed(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb, mlb_process_time* pt, mlb_graph* g,
+                        mlb_buses* b, const int32_t* offsets_host, const mlb_event* events_host, int n_events,
+                        const int32_t* time_offsets_host, const mlb_transport* transports_host, int n_transports,
+                        float* out_host, float* mix_host, float* bus_host, int n_blocks)
 {
   if (!r || !offsets_host) return fail(MLB_ERR_INVALID, "null argument");
   if (b ? (!bus_host || out_host || mix_host) : bus_host != nullptr)
     return fail(MLB_ERR_INVALID, "bus rows come with a bus layout, and then alone (out and mix must be null)");
-  const int n_planes = MLB_VOICE_ROWS + (cb ? cb->C : 0);
+  const int phase_plane = MLB_VOICE_ROWS + (cb ? cb->C : 0);
+  const int n_planes = phase_plane + (pt ? 1 : 0);
   unsigned row_mask;
-  MLB_TRY(synth_check(vb, g, offsets_host, n_blocks, out_host || mix_host || bus_host, &row_mask, n_planes));
+  MLB_TRY(synth_check(vb, g, offsets_host, n_blocks, out_host || mix_host || bus_host, &row_mask, n_planes,
+                      pt != nullptr));
   if (r->V != g->V) return fail(MLB_ERR_INVALID, "router bank writes %d voices, graph has %d", r->V, g->V);
   if ((r->protocol == 0) != ((vb->flags & MLB_VOICES_MIDI) != 0))
     return fail(MLB_ERR_INVALID, "router bank protocol %s, voice bank %s MLB_VOICES_MIDI", r->protocol ? "MPE" : "MIDI",
@@ -3221,8 +3384,18 @@ extern "C" int mlb_synth_process_routed_host(mlb_routers* r, mlb_voices* vb, mlb
     return fail(MLB_ERR_INVALID, "controller bank's voice map has %d voices, graph has %d (mlb_controllers_set_voice_map)",
                 cb->V, g->V);
   if (b && b->V != g->V) return fail(MLB_ERR_INVALID, "buses are laid over %d voices, graph has %d", b->V, g->V);
+  if (pt && pt->G != r->G)
+    return fail(MLB_ERR_INVALID, "router bank has %d instruments, process-time bank %d", r->G, pt->G);
+  if (pt && pt->V != g->V)
+    return fail(MLB_ERR_INVALID,
+                "process-time bank's voice map has %d voices, graph has %d (mlb_process_time_set_voice_map)", pt->V,
+                g->V);
+  if (pt && !time_offsets_host) return fail(MLB_ERR_INVALID, "null transport offsets");
+  if (pt && (n_transports < 0 || (n_transports > 0 && !transports_host)))
+    return fail(MLB_ERR_INVALID, "%d transport updates at %p", n_transports, (const void*)transports_host);
   int n_changes = 0;
   MLB_TRY(routers_check(r, offsets_host, events_host, n_events, n_blocks, &n_changes));
+  if (pt) MLB_TRY(process_time_check_offsets(pt, time_offsets_host, n_transports, n_blocks));
   MLB_TRY(ensure_init());
   const size_t V = (size_t)g->V, T = (size_t)n_blocks, n_out = g->outs.size(), G1 = (size_t)r->G + 1;
   const int Tc = synth_chunk_blocks(g, n_blocks, n_planes);
@@ -3236,6 +3409,8 @@ extern "C" int mlb_synth_process_routed_host(mlb_routers* r, mlb_voices* vb, mlb
   MLB_TRY(r->d_ch.ensure(std::max(n_changes, 1) * sizeof(mlb_controller_change), "staging"));
   MLB_TRY(vb->d_ev.ensure((size_t)Tc * V * sizeof(mlb_voice_events), "staging"));
   MLB_TRY(vb->d_out.ensure((size_t)Tc * n_planes * V * MLB_BLOCK * 4, "staging"));
+  if (pt) MLB_TRY(pt->d_off.ensure(T * G1 * 4, "staging"));
+  if (pt) MLB_TRY(pt->d_tr.ensure(std::max(n_transports, 1) * sizeof(mlb_transport), "staging"));
   const size_t row_floats = n_out * V * MLB_BLOCK;             // output rows per block
   const size_t bus_floats = b ? n_out * b->G * MLB_BLOCK : 0;  // bus rows per block
   float* down_dev = b ? b->d_out.get() : g->d_out.get();
@@ -3253,6 +3428,12 @@ extern "C" int mlb_synth_process_routed_host(mlb_routers* r, mlb_voices* vb, mlb
           if (e == cudaSuccess)
             e = cudaMemcpyAsync(r->d_off.get() + t0 * G1, offsets_host + t0 * G1, (t1 - t0) * G1 * 4,
                                 cudaMemcpyHostToDevice, s);
+          if (e == cudaSuccess && pt && t0 == 0 && n_transports)
+            e = cudaMemcpyAsync(pt->d_tr.get(), transports_host, n_transports * sizeof(mlb_transport),
+                                cudaMemcpyHostToDevice, s);
+          if (e == cudaSuccess && pt)
+            e = cudaMemcpyAsync(pt->d_off.get() + t0 * G1, time_offsets_host + t0 * G1, (t1 - t0) * G1 * 4,
+                                cudaMemcpyHostToDevice, s);
           return e;
         },
         [&](int t0, int t1, cudaStream_t s) -> int
@@ -3263,6 +3444,9 @@ extern "C" int mlb_synth_process_routed_host(mlb_routers* r, mlb_voices* vb, mlb
           if (cb)
             MLB_TRY(mlb_controllers_process_device(cb, r->d_coff.get(), r->d_ch.get(), vb->d_out.get(), MLB_VOICE_ROWS,
                                                    n_planes, t1 - t0, s));
+          if (pt)
+            MLB_TRY(mlb_process_time_process_device(pt, pt->d_off.get() + t0 * G1, pt->d_tr.get(), vb->d_out.get(),
+                                                    phase_plane, n_planes, t1 - t0, s));
           if (b)
           {
             MLB_TRY(graph_process(g, vb->d_out.get(), n_planes, g->d_out.get(), nullptr, t1 - t0, s));
@@ -3282,6 +3466,26 @@ extern "C" int mlb_synth_process_routed_host(mlb_routers* r, mlb_voices* vb, mlb
     return MLB_OK;
   }();
   return drain(rc, {g->s_h2d.get(), g->stream.get(), g->s_d2h.get()});
+}
+
+extern "C" int mlb_synth_process_routed_host(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb, mlb_graph* g,
+                                             mlb_buses* b, const int32_t* offsets_host, const mlb_event* events_host,
+                                             int n_events, float* out_host, float* mix_host, float* bus_host,
+                                             int n_blocks)
+{
+  return synth_routed(r, vb, cb, nullptr, g, b, offsets_host, events_host, n_events, nullptr, nullptr, 0, out_host,
+                      mix_host, bus_host, n_blocks);
+}
+
+extern "C" int mlb_synth_process_context_host(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb,
+                                              mlb_process_time* pt, mlb_graph* g, mlb_buses* b,
+                                              const int32_t* offsets_host, const mlb_event* events_host, int n_events,
+                                              const int32_t* time_offsets_host, const mlb_transport* transports_host,
+                                              int n_transports, float* out_host, float* mix_host, float* bus_host,
+                                              int n_blocks)
+{
+  return synth_routed(r, vb, cb, pt, g, b, offsets_host, events_host, n_events, time_offsets_host, transports_host,
+                      n_transports, out_host, mix_host, bus_host, n_blocks);
 }
 
 // ------------------------------------------------------------------------------------------

@@ -994,3 +994,81 @@ def midi_performance(n_instruments: int, n_blocks: int, polyphony=8, mpe: bool =
                         held[g].clear()
                 i += 1
     return offsets, ev
+
+
+TRANSPORT_CHAOS = ("stop", "jump_back", "negative", "zero", "tempo", "sample_rate", "repeat", "nan", "inf",
+                   "restart")
+
+
+def transport_updates(n_instruments: int, n_blocks: int, sample_rate: float = 48000.0, seed: int = 31,
+                      every: int = 1, chaos: float = 0.0, t0: int = 0):
+    """A host transport per instrument, as a plugin host reports it to AudioContext::updateTime: playing from a
+    random position (0..64 quarter notes) at a random tempo (60..180 bpm), one update before every `every`-th vector
+    (vectors t0, t0 + 1, .. of the song).  With `chaos` > 0, that share of the updates is replaced by one of
+    TRANSPORT_CHAOS (stop, backwards jump, negative or zero position, tempo change, sample-rate change, the previous
+    position again, NaN or infinite position / tempo, a stop followed by a restart from the top at that instrument's
+    next update), and about chaos / 4 of the vectors get no update
+    or two.  Returns (offsets [T][G + 1] int32, transports of api.TRANSPORT_DTYPE), the CSR convention of
+    api.ProcessTimeBank."""
+    G, T = int(n_instruments), int(n_blocks)
+    rng = np.random.default_rng(seed)
+    ppq0 = rng.integers(0, 256, G) * 0.25
+    bpm0 = rng.uniform(60.0, 180.0, G)
+    t = np.arange(T)[:, None] + t0
+    counts = np.broadcast_to((t % every == 0).astype(np.int32), (T, G)).copy()
+    if chaos > 0:
+        r = rng.random((T, G))
+        counts[r < chaos / 8] = 0
+        counts[(r >= chaos / 8) & (r < chaos / 4)] = 2
+    starts = np.zeros(T * G + 1, np.int64)
+    starts[1:] = np.cumsum(counts.reshape(-1))
+    offsets = np.empty((T, G + 1), np.int32)
+    offsets[:, :G] = starts[:-1].reshape(T, G)
+    offsets[:, G] = starts[G::G]
+    n = int(starts[-1])
+    cell = np.repeat(np.arange(T * G), counts.reshape(-1))
+    k = np.arange(n) - starts[cell]
+    tt, g = cell // G + t0, cell % G
+    tr = np.zeros(n, api.TRANSPORT_DTYPE)
+    tr["bpm"] = bpm0[g]
+    tr["ppq_pos"] = ppq0[g] + (tt * 64 + k * 17) * bpm0[g] / (60.0 * sample_rate)
+    tr["sample_rate"] = sample_rate
+    tr["is_playing"] = 1
+    if chaos > 0 and n:
+        # the index of each update's next update of the same instrument (n: none); updates are stored block-major
+        order = np.lexsort((np.arange(n), g))
+        next_same = np.full(n, n)
+        same = g[order[1:]] == g[order[:-1]]
+        next_same[order[:-1][same]] = order[1:][same]
+        hit = np.flatnonzero(rng.random(n) < chaos)
+        kind = rng.integers(0, len(TRANSPORT_CHAOS), hit.size)
+        u = rng.random(hit.size)
+        for j, name in enumerate(TRANSPORT_CHAOS):
+            i, uu = hit[kind == j], u[kind == j]
+            if name == "stop":
+                tr["is_playing"][i] = 0
+            elif name == "jump_back":
+                tr["ppq_pos"][i] -= 0.1 + 4.0 * uu
+            elif name == "negative":
+                tr["ppq_pos"][i] = -3.0 * uu
+            elif name == "zero":
+                tr["ppq_pos"][i] = np.where(uu < 0.5, 0.0, -0.0)
+            elif name == "tempo":
+                tr["bpm"][i] = 40.0 + 200.0 * uu
+            elif name == "sample_rate":
+                tr["sample_rate"][i] = np.where(uu < 0.5, 44100.0, 96000.0)
+            elif name == "repeat":
+                tr["ppq_pos"][i] = tr["ppq_pos"][np.maximum(i - 1, 0)]
+            elif name == "nan":
+                tr["ppq_pos"][i[uu < 0.5]] = np.nan
+                tr["bpm"][i[uu >= 0.5]] = np.nan
+            elif name == "inf":
+                tr["ppq_pos"][i[uu < 0.5]] = np.inf
+                tr["bpm"][i[uu >= 0.5]] = -np.inf
+            elif name == "restart":
+                tr["is_playing"][i] = 0  # then play again from the top of the song at the instrument's next update
+                nxt = next_same[i]
+                nxt = nxt[nxt < n]
+                tr["is_playing"][nxt] = 1
+                tr["ppq_pos"][nxt] = 0.0
+    return offsets, tr

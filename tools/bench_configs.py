@@ -2,14 +2,17 @@
 """Kernel-resident timing of everything except the headline: BASELINE.json configurations 2-5, the
 SURVEY 8(f) workloads (config 6 = Aaltoverb x V, the EventsToSignals::Voice bank) and the elementwise maps.
 
-    python tools/bench_configs.py [--steps K] [--only 2,3,4,5,6,voices,map,fdtd,buses,controllers,router,routed] [--generic] [--cpu]
+    python tools/bench_configs.py [--steps K] [--only 2,3,4,5,6,voices,map,fdtd,buses,controllers,router,routed,
+                                   process_time,context] [--generic] [--cpu]
 
 Prints one JSON line per configuration: kernel name, mean CUDA-event kernel time, algorithmic
 bytes per launch (SURVEY.md 8d / DESIGN.md), achieved GB/s and fraction of the measured HBM peak.
 --cpu also times the reference (oracle/_ref) on the box's host cores for config 6, the Voice bank and the FDTD
 membranes.  The FDTD lines (K9) are compute-bound: they report instance-samples/s and the share of the FP32 issue
 ceiling instead of bytes.  The bus lines (K10) report bytes against the data-sheet HBM bandwidth, and contract E
-with bus output against the rows-out and mix-only paths in voice-samples/s.
+with bus output against the rows-out and mix-only paths in voice-samples/s.  The beat-phase lines (K13) report
+voice-samples/s and bytes against the data-sheet HBM bandwidth, and contract E with every AudioContext signal against
+the routed entry point on the same performance.
 Not the headline benchmark (that is bench.py / config A).
 """
 import argparse
@@ -29,7 +32,8 @@ def main():
     from madronalib_b200 import api, workloads as wl
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
-    ap.add_argument("--only", default="2,3,swept,4,5,6,voices,map,fdtd,buses,controllers,router,routed")
+    ap.add_argument("--only", default="2,3,swept,4,5,6,voices,map,fdtd,buses,controllers,router,routed,process_time,"
+                                      "context")
     ap.add_argument("--generic", action="store_true", help="force the graph interpreter kernel")
     ap.add_argument("--cpu", action="store_true",
                     help="also time the reference (oracle/_ref, all host threads) on config 6, the Voice bank "
@@ -126,6 +130,10 @@ def main():
         bench_router(api, wl, torch, dev, args.steps)
     if "routed" in only:
         bench_routed(api, wl, torch)
+    if "process_time" in only:
+        bench_process_time(api, wl, torch, dev, args.steps)
+    if "context" in only:
+        bench_context(api, wl, torch)
     if args.cpu:
         # the reference itself on this box's host cores (oracle/_ref; checker code, used here only as a baseline)
         import time
@@ -614,6 +622,129 @@ def bench_routed(api, wl, torch, n_calls=5):
     mism = int(((a.view(np.uint32) != b_.view(np.uint32)) & ~(np.isnan(a) & np.isnan(b_))).sum())
     print(json.dumps({"config": "contract_E_routed_parity", "checker": "contract E fed by the host routers",
                       "blocks": T, "mismatches": mism}), flush=True)
+
+
+def bench_process_time(api, wl, torch, dev, steps):
+    """K13 alone, transport updates resident on the device: 4 096 instruments x 64 vectors of a steady host transport
+    (one update per vector), as instrument rows and through a 65 536-voice map (16 voices each), mean of `steps`
+    CUDA-event-timed calls after 2 warm-up calls.  Bytes = the rows written (the updates read are 0.05 % of them).
+    Parity of a fresh bank's first call against the port (oracle/port/mlport_ptime.c), every row."""
+    from oracle.ptime_bindings import port_process_time
+    G, P, T, sr = 4096, 16, 64, 48000.0
+    facts = gpu_facts()
+    lay = wl.midi_layout(G, P)
+    offsets, tr = wl.transport_updates(G, T, sr, seed=60)
+    want, _ = port_process_time(G, offsets, tr, sr)
+    d_off = torch.from_numpy(offsets).to(dev)
+    d_tr = torch.from_numpy(tr.view(np.uint8)).to(dev)
+    sh = torch.cuda.current_stream().cuda_stream
+    for vmap in (None, lay["voice_instrument"]):
+        N = G if vmap is None else lay["n_voices"]
+        d_out = torch.empty((T, 1, N, 64), dtype=torch.float32, device=dev)
+        pt = api.ProcessTimeBank(G, sr)
+        pt.set_voice_map(vmap)
+        w0 = pt.get_state()
+        pt.process_device(d_off, d_tr, d_out, T, stream=sh)
+        torch.cuda.synchronize()
+        got = d_out[:, 0].cpu().numpy()
+        ref = want if vmap is None else want[:, vmap]
+        mism = int(((got.view(np.uint32) != ref.view(np.uint32)) & ~(np.isnan(got) & np.isnan(ref))).sum())
+        for _ in range(2):
+            pt.set_state(w0)
+            pt.process_device(d_off, d_tr, d_out, T, stream=sh)
+        pt.set_state(w0)
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(steps):
+            pt.process_device(d_off, d_tr, d_out, T, stream=sh)
+        e1.record()
+        torch.cuda.synchronize()
+        ms = e0.elapsed_time(e1) / steps
+        pt.close()
+        nbytes = 256.0 * N * T
+        print(json.dumps({
+            "config": "process_time_%dx%d_%s" % (G, T, "instrument_rows" if vmap is None else "voice_map_%d" % N),
+            "kernel": "process_time_kernel", "instruments": G, "rows": N, "blocks": T, "ms_per_call": ms,
+            "voice_samples_per_s": N * T * 64 / (ms * 1e-3), "row_bytes_written": nbytes,
+            "achieved_gbs": nbytes / (ms * 1e-3) / 1e9,
+            "frac_of_datasheet_hbm": nbytes / (ms * 1e-3) / 1e9 / HBM_DATASHEET_GBS,
+            "datasheet_note": "3.35 TB/s, H100 SXM data sheet", **facts,
+            "parity_checker": "oracle/port/mlport_ptime.c", "mismatched_words": mism}), flush=True)
+        del d_out
+
+
+def bench_context(api, wl, torch, n_calls=5):
+    """Contract E with every AudioContext signal (mlb_synth_process_context_host: routers, Voice rows, controllers 1
+    and 74, the beat phase, config A, bus rows out) against the routed entry point on the same performance (4 096
+    instruments x 16 voices x 64 vectors of midi_performance, one transport update per instrument and vector), pinned
+    host buffers, host clock around calls that return finished, the two alternated.  Config A reads only the Voice
+    rows, so the bus rows of the two paths must match bit for bit; the difference in time is K11 + K13."""
+    import time
+    from madronalib_b200.api import EVENT_DTYPE, TRANSPORT_DTYPE
+    G, P, T, sr = 4096, 16, 64, 48000.0
+    facts = gpu_facts()
+    lay = wl.midi_layout(G, P)
+    V = lay["n_voices"]
+    w = wl.config_a(V)
+    vi, gs, da, pb = wl.synth_bank_params(V)
+    offsets, ev = wl.midi_performance(G, T, P, density=0.1, seed=51)
+    toff, tr = wl.transport_updates(G, T, sr, seed=61)
+    L = api.lib()
+
+    def pinned(a, dtype):
+        p = torch.empty((max(a.nbytes, 1),), dtype=torch.uint8).pin_memory().numpy()
+        p[:a.nbytes] = np.ascontiguousarray(a).view(np.uint8).reshape(-1)
+        return p[:a.nbytes].view(dtype).reshape(a.shape)
+
+    ev_pin, off_pin = pinned(ev, EVENT_DTYPE), pinned(offsets, np.int32)
+    tr_pin, toff_pin = pinned(tr, TRANSPORT_DTYPE), pinned(toff, np.int32)
+    h_bus = {k: torch.empty((T, 1, G, 64), dtype=torch.float32).pin_memory().numpy() for k in ("routed", "context")}
+    hs = {}
+    for name in ("routed", "context"):
+        vb = api.VoiceBank(sr, lay["voice_index"], gs, da, pb, flags=api.VoiceBank.MIDI)
+        g = api.VoiceGraph(w.spec, V)
+        g.set_coefs(w.coef)
+        g.set_state(w.state)
+        b = api.Buses(V, lay["bus_first"], lay["bus_count"])
+        r = api.RouterBank(lay["polyphony"], lay["first_voice"], V)
+        cb = api.ControllerBank(G, [1, 74], sr)
+        cb.set_voice_map(lay["voice_instrument"])
+        pt = api.ProcessTimeBank(G, sr)
+        pt.set_voice_map(lay["voice_instrument"])
+        hs[name] = (vb, g, b, r, cb, pt)
+    out_first = {}
+
+    def call(name):
+        vb, g, b, r, cb, pt = hs[name]
+        out = h_bus[name]
+        if name == "routed":
+            return L.mlb_synth_process_routed_host(r._h, vb._h, None, g._h, b._h, off_pin.ctypes.data,
+                                                   ev_pin.ctypes.data, int(ev.size), None, None, out.ctypes.data, T)
+        return L.mlb_synth_process_context_host(r._h, vb._h, cb._h, pt._h, g._h, b._h, off_pin.ctypes.data,
+                                                ev_pin.ctypes.data, int(ev.size), toff_pin.ctypes.data,
+                                                tr_pin.ctypes.data, int(tr.size), None, None, out.ctypes.data, T)
+
+    for name in hs:
+        assert call(name) == 0, L.mlb_last_error()
+        out_first[name] = h_bus[name].copy()
+    dt = {k: 0.0 for k in hs}
+    for _ in range(n_calls):
+        for name in hs:
+            t0 = time.perf_counter()
+            call(name)
+            dt[name] += (time.perf_counter() - t0) / n_calls
+    for hh in hs.values():
+        for h in hh:
+            h.close()
+    for name in hs:
+        print(json.dumps({"config": "context_pair_%s_buses" % name, "instruments": G, "voices": V, "blocks": T,
+                          "events": int(ev.size), "transport_updates": int(tr.size) if name == "context" else 0,
+                          "planes": 8 + (3 if name == "context" else 0), "ms_per_call": 1e3 * dt[name],
+                          "voice_samples_per_s": V * T * 64 / dt[name], **facts}), flush=True)
+    a, b_ = out_first["routed"], out_first["context"]
+    mism = int(((a.view(np.uint32) != b_.view(np.uint32)) & ~(np.isnan(a) & np.isnan(b_))).sum())
+    print(json.dumps({"config": "contract_E_context_parity", "checker": "the routed entry point", "blocks": T,
+                      "mismatches": mism}), flush=True)
 
 
 if __name__ == "__main__":
