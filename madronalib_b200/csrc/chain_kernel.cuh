@@ -256,7 +256,10 @@ __global__ void __launch_bounds__(kChainMaxWarps * 32)
     mbar_arrive_expect_tx(bar, (uint32_t)P::NP * kBlockBytes);
     const uint32_t dst = blocks + (uint32_t)ld_stage * kStageBytes;
     const int z0 = (u.t0 + ld_blk) * a.n_in_planes;
-    if (P::HAS_IN) tma_load_4d(dst, &in_map, bar, 0, u.g * kTileVoices, 0, z0 + a.in_plane, kEvictFirst);
+    // The input rows are read once, yet they stream faster with an evict-last hint than with evict-first or
+    // evict-normal: 0.776 / 0.800 / 0.788 ms for config A on an H100 SXM at 700 W (DESIGN.md 7).  The hint only
+    // changes which lines L2 gives up first; why that helps the write-backs of the output rows is not measured.
+    if (P::HAS_IN) tma_load_4d(dst, &in_map, bar, 0, u.g * kTileVoices, 0, z0 + a.in_plane, kEvictLast);
 #pragma unroll
     for (int p = 0; p < P::NV; ++p)
       tma_load_4d(dst + (uint32_t)((P::HAS_IN ? 1 : 0) + p) * kBlockBytes, &in_map, bar, 0, u.g * kTileVoices, 0,

@@ -157,6 +157,7 @@ __device__ __forceinline__ void prefetch_tensormap(const CUtensorMap* map)
 // L2 eviction-priority hints for streaming data (values as used by CUTLASS' TMA::CacheHintSm90)
 constexpr uint64_t kEvictFirst = 0x12F0000000000000ull;
 constexpr uint64_t kEvictNormal = 0x1000000000000000ull;
+constexpr uint64_t kEvictLast = 0x14F0000000000000ull;
 
 __device__ __forceinline__ float4 lds128(uint32_t addr)
 {
