@@ -404,25 +404,44 @@ class VoiceGraph(_Handle):
                                             _ptr(mix) if want_mix else None, T))
         return out, mix
 
+    def _contract_e(self, name: str, events=None, offsets=None, n_instruments: int = 0, buses=None,
+                    want_out: bool = False, want_mix: bool = False, out=None, mix=None):
+        """The arguments of a contract-E call: checks the records `events` [T][V], or the offsets
+        [T][n_instruments + 1] (returned as int32); then allocates the arrays asked for and not given, and checks those
+        given, which C writes in place: `out` the rows [T][n_out][V][64], or with `buses` the bus rows
+        [T][n_out][G][64] (asked for always, no mix bus), and `mix` [T][n_out][64].  Returns (T, offsets, out, mix)."""
+        s, V = self.spec, self.n_voices
+        if offsets is None:
+            if not (isinstance(events, np.ndarray) and events.ndim == 2 and events.shape[1] == V and
+                    events.dtype.itemsize == 72 and events.flags["C_CONTIGUOUS"]):
+                raise ValueError(f"{name}: `events` must be a C-contiguous [T][V] array of 72-byte records")
+            T = int(events.shape[0])
+        else:
+            offsets = np.ascontiguousarray(offsets, np.int32)
+            if offsets.ndim != 2 or offsets.shape[1] != n_instruments + 1:
+                raise ValueError(f"{name}: offsets must be [T][{n_instruments + 1}], got {offsets.shape}")
+            T = int(offsets.shape[0])
+        shape = (T, s.n_out, V, BLOCK)
+        if buses is not None:
+            shape, want_out, want_mix = (T, s.n_out, buses.n_buses, BLOCK), True, False
+        if want_out and out is None:
+            out = np.empty(shape, np.float32)
+        if want_mix and mix is None:
+            mix = np.empty((T, s.n_out, BLOCK), np.float32)
+        for key, a, shp in (("out", out if want_out else None, shape),
+                            ("mix", mix if want_mix else None, (T, s.n_out, BLOCK))):
+            if a is not None and not (isinstance(a, np.ndarray) and a.dtype == np.float32 and
+                                      a.flags["C_CONTIGUOUS"] and a.shape == shp):
+                raise ValueError(f"{name}: `{key}` must be a C-contiguous float32 array of shape {shp}")
+        return T, offsets, out, mix
+
     def process_events_host(self, bank: "VoiceBank", events: np.ndarray, want_out: bool = True,
                             want_mix: bool = False, out: Optional[np.ndarray] = None,
                             mix: Optional[np.ndarray] = None):
         """Contract E (mlb_synth_process_host): event records [T][V] in, the graph's rows / mix bus out.
         The graph's INPUT plane r is Voice row r of ``bank``; the rows never leave the device."""
-        s, V = self.spec, self.n_voices
-        if not (isinstance(events, np.ndarray) and events.ndim == 2 and events.shape[1] == V and
-                events.dtype.itemsize == 72 and events.flags["C_CONTIGUOUS"]):
-            raise ValueError("process_events_host: `events` must be a C-contiguous [T][V] array of 72-byte records")
-        T = int(events.shape[0])
-        if want_out and out is None:
-            out = np.empty((T, s.n_out, V, BLOCK), np.float32)
-        if want_mix and mix is None:
-            mix = np.empty((T, s.n_out, BLOCK), np.float32)
-        for name, a, shape in (("out", out if want_out else None, (T, s.n_out, V, BLOCK)),
-                               ("mix", mix if want_mix else None, (T, s.n_out, BLOCK))):
-            if a is not None and not (isinstance(a, np.ndarray) and a.dtype == np.float32 and
-                                      a.flags["C_CONTIGUOUS"] and a.shape == shape):
-                raise ValueError(f"process_events_host: `{name}` must be a C-contiguous float32 array of shape {shape}")
+        T, _, out, mix = self._contract_e("process_events_host", events, want_out=want_out, want_mix=want_mix,
+                                          out=out, mix=mix)
         _check(lib().mlb_synth_process_host(bank._h, self._h, events.ctypes.data,
                                             _ptr(out) if want_out else None,
                                             _ptr(mix) if want_mix else None, T))
@@ -435,19 +454,12 @@ class VoiceGraph(_Handle):
         change list (offsets [T][G + 1], changes) in, the graph's rows / mix bus out.  INPUT planes 0..7 are the
         Voice rows of ``bank``, plane 8 + k controller k of ``controllers`` (which needs a voice map of this graph's
         voices); nothing but records and changes crosses PCIe on the way in."""
-        s, V = self.spec, self.n_voices
-        if not (isinstance(events, np.ndarray) and events.ndim == 2 and events.shape[1] == V and
-                events.dtype.itemsize == 72 and events.flags["C_CONTIGUOUS"]):
-            raise ValueError("process_events_controllers_host: `events` must be a C-contiguous [T][V] array of 72-byte "
-                             "records")
-        T = int(events.shape[0])
+        name = "process_events_controllers_host"
+        T, _, out, mix = self._contract_e(name, events, want_out=want_out, want_mix=want_mix)
         off = np.ascontiguousarray(offsets, np.int32)
         if off.shape != (T, controllers.n_instruments + 1):
-            raise ValueError(f"process_events_controllers_host: offsets must be [{T}][{controllers.n_instruments + 1}], "
-                             f"got {off.shape}")
+            raise ValueError(f"{name}: offsets must be [{T}][{controllers.n_instruments + 1}], got {off.shape}")
         ch = np.ascontiguousarray(changes, CONTROLLER_CHANGE_DTYPE)
-        out = np.empty((T, s.n_out, V, BLOCK), np.float32) if want_out else None
-        mix = np.empty((T, s.n_out, BLOCK), np.float32) if want_mix else None
         _check(lib().mlb_synth_process_controllers_host(bank._h, controllers._h, self._h, events.ctypes.data,
                                                         off.ctypes.data, ch.ctypes.data if ch.size else None,
                                                         _ptr(out), _ptr(mix), T))
@@ -458,18 +470,7 @@ class VoiceGraph(_Handle):
         """Contract E with per-instrument output (mlb_synth_process_buses_host): event records [T][V] in, the bus rows
         [T][n_out][G][64] out -- each bus the strict-order sum of its voices' output rows (Synth::processVector).
         The voice rows never leave the device."""
-        s, V = self.spec, self.n_voices
-        if not (isinstance(events, np.ndarray) and events.ndim == 2 and events.shape[1] == V and
-                events.dtype.itemsize == 72 and events.flags["C_CONTIGUOUS"]):
-            raise ValueError("process_events_buses_host: `events` must be a C-contiguous [T][V] array of 72-byte "
-                             "records")
-        T = int(events.shape[0])
-        shape = (T, s.n_out, buses.n_buses, BLOCK)
-        if out is None:
-            out = np.empty(shape, np.float32)
-        if not (isinstance(out, np.ndarray) and out.dtype == np.float32 and out.flags["C_CONTIGUOUS"] and
-                out.shape == shape):
-            raise ValueError(f"process_events_buses_host: `out` must be a C-contiguous float32 array of shape {shape}")
+        T, _, out, _ = self._contract_e("process_events_buses_host", events, buses=buses, out=out)
         _check(lib().mlb_synth_process_buses_host(bank._h, self._h, buses._h, events.ctypes.data, _ptr(out), T))
         return out
 
@@ -480,18 +481,11 @@ class VoiceGraph(_Handle):
         routed on the device by ``routers``, then the Voice rows of ``bank``, the controller planes of ``controllers``
         (if given) and this graph.  Without ``buses``: returns (out [T][n_out][V][64] or None, mix [T][n_out][64] or
         None); with ``buses``: returns the bus rows [T][n_out][G_bus][64]."""
-        s, V = self.spec, self.n_voices
-        off = np.ascontiguousarray(offsets, np.int32)
-        if off.ndim != 2 or off.shape[1] != routers.n_instruments + 1:
-            raise ValueError(f"process_routed_host: offsets must be [T][{routers.n_instruments + 1}], got {off.shape}")
+        T, off, out, mix = self._contract_e("process_routed_host", offsets=offsets,
+                                            n_instruments=routers.n_instruments, buses=buses, want_out=want_out,
+                                            want_mix=want_mix)
         ev = np.ascontiguousarray(events, EVENT_DTYPE)
-        T = int(off.shape[0])
-        out = mix = bus = None
-        if buses is not None:
-            bus = np.empty((T, s.n_out, buses.n_buses, BLOCK), np.float32)
-        else:
-            out = np.empty((T, s.n_out, V, BLOCK), np.float32) if want_out else None
-            mix = np.empty((T, s.n_out, BLOCK), np.float32) if want_mix else None
+        bus, out = (out, None) if buses is not None else (None, out)
         _check(lib().mlb_synth_process_routed_host(routers._h, bank._h, controllers._h if controllers else None, self._h,
                                                    buses._h if buses else None, off.ctypes.data,
                                                    ev.ctypes.data if ev.size else None, int(ev.size), _ptr(out),
@@ -506,12 +500,10 @@ class VoiceGraph(_Handle):
         beat phase of ``times`` (if given) fed by time_offsets [T][G + 1] into transports (TRANSPORT_DTYPE).  The
         graph's INPUT planes are the 8 Voice rows, then the controller planes, then the beat phase.  Returns as
         process_routed_host."""
-        s, V = self.spec, self.n_voices
-        off = np.ascontiguousarray(offsets, np.int32)
-        if off.ndim != 2 or off.shape[1] != routers.n_instruments + 1:
-            raise ValueError(f"process_context_host: offsets must be [T][{routers.n_instruments + 1}], got {off.shape}")
+        T, off, out, mix = self._contract_e("process_context_host", offsets=offsets,
+                                            n_instruments=routers.n_instruments, buses=buses, want_out=want_out,
+                                            want_mix=want_mix)
         ev = np.ascontiguousarray(events, EVENT_DTYPE)
-        T = int(off.shape[0])
         toff = tr = None
         if times is not None:
             if time_offsets is None or transports is None:
@@ -520,12 +512,7 @@ class VoiceGraph(_Handle):
             if toff.shape != off.shape:
                 raise ValueError(f"process_context_host: time_offsets must be {off.shape}, got {toff.shape}")
             tr = np.ascontiguousarray(transports, TRANSPORT_DTYPE)
-        out = mix = bus = None
-        if buses is not None:
-            bus = np.empty((T, s.n_out, buses.n_buses, BLOCK), np.float32)
-        else:
-            out = np.empty((T, s.n_out, V, BLOCK), np.float32) if want_out else None
-            mix = np.empty((T, s.n_out, BLOCK), np.float32) if want_mix else None
+        bus, out = (out, None) if buses is not None else (None, out)
         _check(lib().mlb_synth_process_context_host(
             routers._h, bank._h, controllers._h if controllers else None, times._h if times else None, self._h,
             buses._h if buses else None, off.ctypes.data, ev.ctypes.data if ev.size else None, int(ev.size),

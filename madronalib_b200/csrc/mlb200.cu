@@ -2528,10 +2528,12 @@ extern "C" int mlb_voices_process_host(mlb_voices* vb, const mlb_voice_events* e
 // Pipelined over TIME chunks by host_pipeline -- blocks are contiguous in every buffer involved, and both
 // the bank and the graph carry their state from launch to launch -- so that the H2D copy of chunk c+1's
 // records, the kernels of chunk c and the D2H copy of chunk c-1's output rows overlap.
-// mlb_synth_process_buses_host runs the same pipeline with the bus kernel (K10) after the graph.
+// All five contract-E entry points (records, buses, controllers, routed, context) run their own checks, describe the
+// call in a SynthCall and hand it to the one driver, SynthCall::run (defined after the banks it runs): per chunk the
+// router (K12) from raw events, the voice kernel, K11 and K13 if given, the graph, and the bus sum (K10) if given.
 
-// The checks both contract-E entry points share; *row_mask = the Voice rows the graph reads.
-// n_planes: the input planes per block, the 8 Voice rows and any controller planes after them.
+// The checks every contract-E entry point shares; *row_mask = the Voice rows the graph reads.
+// n_planes: the input planes per block, the 8 Voice rows and any controller planes and beat phase after them.
 // events_host: the records, or the raw events' offsets of the routed entry point.
 static int synth_check(const mlb_voices* vb, const mlb_graph* g, const void* events_host, int n_blocks,
                        bool wants_output, unsigned* row_mask, int n_planes = MLB_VOICE_ROWS, bool phase_plane = false)
@@ -2569,45 +2571,41 @@ static int synth_chunk_blocks(const mlb_graph* g, int n_blocks, int n_planes = M
   return std::max<int>(Tc, (n_blocks + mlb_graph::kMaxHostSlices - 1) / mlb_graph::kMaxHostSlices);
 }
 
+// One checked contract-E call.  The records come from the host (`records`) or from the router bank `r` (raw events);
+// the controller changes of `cb` from the router, or without one from the host (`ctrl_offsets` into `ctrl_changes`).
+// Out rows and / or the mix bus come back, or the bus rows of `b` alone.
+struct SynthCall
+{
+  mlb_voices* vb = nullptr;
+  mlb_graph* g = nullptr;
+  unsigned row_mask = 0;          // the Voice rows the graph reads
+  int n_planes = MLB_VOICE_ROWS;  // input planes per block: the Voice rows, the controller planes, the beat phase
+  int n_blocks = 0;
+  const mlb_voice_events* records = nullptr;  // [T][V]
+  mlb_routers* r = nullptr;
+  const int32_t* offsets = nullptr;  // [T][G + 1] into events
+  const mlb_event* events = nullptr;
+  int n_events = 0;
+  int n_changes = 0;  // the controller changes the router makes, or those the host uploads
+  mlb_controllers* cb = nullptr;
+  const int32_t* ctrl_offsets = nullptr;  // [T][G + 1] into ctrl_changes
+  const mlb_controller_change* ctrl_changes = nullptr;
+  mlb_process_time* pt = nullptr;         // the beat phase, the last input plane
+  const int32_t* time_offsets = nullptr;  // [T][G + 1] into transports
+  const mlb_transport* transports = nullptr;
+  int n_transports = 0;
+  mlb_buses* b = nullptr;
+  float *out = nullptr, *mix = nullptr, *bus = nullptr;
+  int run() const;  // the driver
+};
+
 extern "C" int mlb_synth_process_host(mlb_voices* vb, mlb_graph* g, const mlb_voice_events* events_host,
                                       float* out_host, float* mix_host, int n_blocks)
 {
-  unsigned row_mask;
-  MLB_TRY(synth_check(vb, g, events_host, n_blocks, out_host || mix_host, &row_mask));
-  MLB_TRY(ensure_init());
-  const size_t V = (size_t)g->V, T = (size_t)n_blocks, n_out = g->outs.size();
-  const int Tc = synth_chunk_blocks(g, n_blocks);
-  if (out_host) MLB_TRY(g->d_out.ensure(T * n_out * V * MLB_BLOCK * 4, "staging"));
-  if (mix_host) MLB_TRY(g->d_mix.ensure(T * n_out * MLB_BLOCK * 4, "staging"));
-  MLB_TRY(vb->d_ev.ensure(T * V * sizeof(mlb_voice_events), "staging"));
-  MLB_TRY(vb->d_out.ensure((size_t)Tc * MLB_VOICE_ROWS * V * MLB_BLOCK * 4, "staging"));
-  const size_t row_floats = n_out * V * MLB_BLOCK;  // output rows per block
-  const int rc = [&]() -> int
-  {
-    MLB_TRY(host_pipeline(
-        g, n_blocks, Tc, true, out_host != nullptr,
-        [&](int t0, int t1, cudaStream_t s)
-        {
-          return cudaMemcpyAsync(vb->d_ev.get() + t0 * V, events_host + t0 * V, (t1 - t0) * V * sizeof(mlb_voice_events),
-                                 cudaMemcpyHostToDevice, s);
-        },
-        [&](int t0, int t1, cudaStream_t s) -> int
-        {
-          MLB_TRY(mlb_voices_process_device(vb, vb->d_ev.get() + t0 * V, vb->d_out.get(), t1 - t0, row_mask, s));
-          return graph_process(g, vb->d_out.get(), MLB_VOICE_ROWS, out_host ? g->d_out.get() + t0 * row_floats : nullptr,
-                               mix_host ? g->d_mix.get() + t0 * n_out * MLB_BLOCK : nullptr, t1 - t0, s);
-        },
-        [&](int t0, int t1, cudaStream_t s)
-        {
-          return cudaMemcpyAsync(out_host + t0 * row_floats, g->d_out.get() + t0 * row_floats,
-                                 (t1 - t0) * row_floats * 4, cudaMemcpyDeviceToHost, s);
-        }));
-    if (mix_host) MLB_TRY(mlb_graph_mix_wait(g, g->stream.get()));
-    if (mix_host)
-      CU_CHECK(cudaMemcpyAsync(mix_host, g->d_mix.get(), T * n_out * MLB_BLOCK * 4, cudaMemcpyDeviceToHost, g->stream.get()));
-    return MLB_OK;
-  }();
-  return drain(rc, {g->s_h2d.get(), g->stream.get(), g->s_d2h.get()});
+  SynthCall c;
+  MLB_TRY(synth_check(vb, g, events_host, n_blocks, out_host || mix_host, &c.row_mask));
+  c.vb = vb, c.g = g, c.n_blocks = n_blocks, c.records = events_host, c.out = out_host, c.mix = mix_host;
+  return c.run();
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2676,37 +2674,12 @@ extern "C" int mlb_buses_sum_device(mlb_buses* b, const float* rows_dev, float* 
 extern "C" int mlb_synth_process_buses_host(mlb_voices* vb, mlb_graph* g, mlb_buses* b,
                                             const mlb_voice_events* events_host, float* bus_host, int n_blocks)
 {
-  unsigned row_mask;
-  MLB_TRY(synth_check(vb, g, events_host, n_blocks, true, &row_mask));
+  SynthCall c;
+  MLB_TRY(synth_check(vb, g, events_host, n_blocks, true, &c.row_mask));
   if (!b || !bus_host) return fail(MLB_ERR_INVALID, "null argument");
   if (b->V != g->V) return fail(MLB_ERR_INVALID, "buses are laid over %d voices, graph has %d", b->V, g->V);
-  MLB_TRY(ensure_init());
-  const size_t V = (size_t)g->V, T = (size_t)n_blocks, n_out = g->outs.size(), G = (size_t)b->G;
-  const int Tc = synth_chunk_blocks(g, n_blocks);
-  MLB_TRY(g->d_out.ensure((size_t)Tc * n_out * V * MLB_BLOCK * 4, "staging"));
-  MLB_TRY(b->d_out.ensure(T * n_out * G * MLB_BLOCK * 4, "staging"));
-  MLB_TRY(vb->d_ev.ensure(T * V * sizeof(mlb_voice_events), "staging"));
-  MLB_TRY(vb->d_out.ensure((size_t)Tc * MLB_VOICE_ROWS * V * MLB_BLOCK * 4, "staging"));
-  const size_t bus_floats = n_out * G * MLB_BLOCK;  // bus rows per block
-  const int rc = host_pipeline(
-      g, n_blocks, Tc, true, true,
-      [&](int t0, int t1, cudaStream_t s)
-      {
-        return cudaMemcpyAsync(vb->d_ev.get() + t0 * V, events_host + t0 * V, (t1 - t0) * V * sizeof(mlb_voice_events),
-                               cudaMemcpyHostToDevice, s);
-      },
-      [&](int t0, int t1, cudaStream_t s) -> int
-      {
-        MLB_TRY(mlb_voices_process_device(vb, vb->d_ev.get() + t0 * V, vb->d_out.get(), t1 - t0, row_mask, s));
-        MLB_TRY(graph_process(g, vb->d_out.get(), MLB_VOICE_ROWS, g->d_out.get(), nullptr, t1 - t0, s));
-        return mlb_buses_sum_device(b, g->d_out.get(), b->d_out.get() + t0 * bus_floats, (int)n_out, t1 - t0, s);
-      },
-      [&](int t0, int t1, cudaStream_t s)
-      {
-        return cudaMemcpyAsync(bus_host + t0 * bus_floats, b->d_out.get() + t0 * bus_floats, (t1 - t0) * bus_floats * 4,
-                               cudaMemcpyDeviceToHost, s);
-      });
-  return drain(rc, {g->s_h2d.get(), g->stream.get(), g->s_d2h.get()});
+  c.vb = vb, c.g = g, c.n_blocks = n_blocks, c.records = events_host, c.b = b, c.bus = bus_host;
+  return c.run();
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2875,18 +2848,30 @@ extern "C" int mlb_controllers_process_device(mlb_controllers* cb, const int32_t
   return MLB_OK;
 }
 
-// offsets [T][G + 1] must index changes of n_changes entries, non-decreasing within each block
-static int controllers_check_offsets(const mlb_controllers* cb, const int32_t* offsets, int n_changes, int n_blocks)
+// offsets [T][G + 1] of the controller changes, transport updates and raw events must index a list of n_items entries,
+// non-decreasing within each block; the message names the range (`what`) and the list's entries (`items`).
+// each(t, g, i0, i1) checks the entries of a range right after the range itself (in the same pass: the host walks
+// these tables on every call).
+template <class Each>
+static int check_offsets(const int32_t* offsets, int G, int n_items, int n_blocks, const char* what, const char* items,
+                         Each each)
 {
   for (int t = 0; t < n_blocks; ++t)
   {
-    const int32_t* o = offsets + (size_t)t * (cb->G + 1);
-    for (int g = 0; g < cb->G; ++g)
-      if (o[g] < 0 || o[g] > o[g + 1] || o[g + 1] > n_changes)
-        return fail(MLB_ERR_INVALID, "block %d, instrument %d: change range [%d, %d) is not within the %d changes", t,
-                    g, o[g], o[g + 1], n_changes);
+    const int32_t* o = offsets + (size_t)t * (G + 1);
+    for (int g = 0; g < G; ++g)
+    {
+      if (o[g] < 0 || o[g] > o[g + 1] || o[g + 1] > n_items)
+        return fail(MLB_ERR_INVALID, "block %d, instrument %d: %s range [%d, %d) is not within the %d %s", t, g, what,
+                    o[g], o[g + 1], n_items, items);
+      MLB_TRY(each(t, g, o[g], o[g + 1]));
+    }
   }
   return MLB_OK;
+}
+static int check_offsets(const int32_t* offsets, int G, int n_items, int n_blocks, const char* what, const char* items)
+{
+  return check_offsets(offsets, G, n_items, n_blocks, what, items, [](int, int, int, int) { return MLB_OK; });
 }
 
 extern "C" int mlb_controllers_process_host(mlb_controllers* cb, const int32_t* offsets_host,
@@ -2896,7 +2881,7 @@ extern "C" int mlb_controllers_process_host(mlb_controllers* cb, const int32_t* 
   if (!cb || !offsets_host || !out_host || (n_changes > 0 && !changes_host)) return fail(MLB_ERR_INVALID, "null argument");
   if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive (got %d)", n_blocks);
   if (n_changes < 0) return fail(MLB_ERR_INVALID, "n_changes must not be negative (got %d)", n_changes);
-  MLB_TRY(controllers_check_offsets(cb, offsets_host, n_changes, n_blocks));
+  MLB_TRY(check_offsets(offsets_host, cb->G, n_changes, n_blocks, "change", "changes"));
   if (plane0 < 0 || n_planes < plane0 + cb->C)
     return fail(MLB_ERR_INVALID, "planes [%d, %d) of the %d controllers are not within the %d output planes", plane0,
                 plane0 + cb->C, cb->C, n_planes);
@@ -2924,18 +2909,16 @@ extern "C" int mlb_controllers_process_host(mlb_controllers* cb, const int32_t* 
 }
 
 // Contract E with controller planes: the graph's input per block is the 8 Voice rows, then the C controller rows
-// in the bank's list order.  Per time chunk on the pipeline of mlb_synth_process_host: records and offsets go up on
-// s_h2d (all changes with the first chunk), the voice kernel, K11 and the graph run on the graph's stream, output rows
-// come down on s_d2h.
+// in the bank's list order; the records and the change offsets go up per chunk, all changes with the first chunk.
 extern "C" int mlb_synth_process_controllers_host(mlb_voices* vb, mlb_controllers* cb, mlb_graph* g,
                                                   const mlb_voice_events* events_host, const int32_t* ctrl_offsets_host,
                                                   const mlb_controller_change* ctrl_changes_host, float* out_host,
                                                   float* mix_host, int n_blocks)
 {
   if (!cb || !ctrl_offsets_host) return fail(MLB_ERR_INVALID, "null argument");
-  const int n_planes = MLB_VOICE_ROWS + cb->C;
-  unsigned row_mask;
-  MLB_TRY(synth_check(vb, g, events_host, n_blocks, out_host || mix_host, &row_mask, n_planes));
+  SynthCall c;
+  c.n_planes = MLB_VOICE_ROWS + cb->C;
+  MLB_TRY(synth_check(vb, g, events_host, n_blocks, out_host || mix_host, &c.row_mask, c.n_planes));
   if (cb->V != g->V)
     return fail(MLB_ERR_INVALID, "controller bank's voice map has %d voices, graph has %d (mlb_controllers_set_voice_map)",
                 cb->V, g->V);
@@ -2945,54 +2928,10 @@ extern "C" int mlb_synth_process_controllers_host(mlb_voices* vb, mlb_controller
   int n_changes = 0;  // the changes the offsets index
   for (int t = 0; t < n_blocks; ++t) n_changes = std::max(n_changes, ctrl_offsets_host[(size_t)t * (cb->G + 1) + cb->G]);
   if (n_changes > 0 && !ctrl_changes_host) return fail(MLB_ERR_INVALID, "null controller changes");
-  MLB_TRY(controllers_check_offsets(cb, ctrl_offsets_host, n_changes, n_blocks));
-  MLB_TRY(ensure_init());
-  const size_t V = (size_t)g->V, T = (size_t)n_blocks, n_out = g->outs.size(), G1 = (size_t)cb->G + 1;
-  const int Tc = synth_chunk_blocks(g, n_blocks, n_planes);
-  if (out_host) MLB_TRY(g->d_out.ensure(T * n_out * V * MLB_BLOCK * 4, "staging"));
-  if (mix_host) MLB_TRY(g->d_mix.ensure(T * n_out * MLB_BLOCK * 4, "staging"));
-  MLB_TRY(vb->d_ev.ensure(T * V * sizeof(mlb_voice_events), "staging"));
-  MLB_TRY(vb->d_out.ensure((size_t)Tc * n_planes * V * MLB_BLOCK * 4, "staging"));
-  MLB_TRY(cb->d_off.ensure(T * G1 * 4, "staging"));
-  if (n_changes) MLB_TRY(cb->d_ch.ensure((size_t)n_changes * sizeof(mlb_controller_change), "staging"));
-  const size_t row_floats = n_out * V * MLB_BLOCK;  // output rows per block
-  const int rc = [&]() -> int
-  {
-    MLB_TRY(host_pipeline(
-        g, n_blocks, Tc, true, out_host != nullptr,
-        [&](int t0, int t1, cudaStream_t s)
-        {
-          cudaError_t e = cudaSuccess;
-          if (t0 == 0 && n_changes)
-            e = cudaMemcpyAsync(cb->d_ch.get(), ctrl_changes_host, (size_t)n_changes * sizeof(mlb_controller_change),
-                                cudaMemcpyHostToDevice, s);
-          if (e == cudaSuccess)
-            e = cudaMemcpyAsync(cb->d_off.get() + t0 * G1, ctrl_offsets_host + t0 * G1, (t1 - t0) * G1 * 4,
-                                cudaMemcpyHostToDevice, s);
-          if (e == cudaSuccess)
-            e = cudaMemcpyAsync(vb->d_ev.get() + t0 * V, events_host + t0 * V, (t1 - t0) * V * sizeof(mlb_voice_events),
-                                cudaMemcpyHostToDevice, s);
-          return e;
-        },
-        [&](int t0, int t1, cudaStream_t s) -> int
-        {
-          MLB_TRY(voices_launch(vb, vb->d_ev.get() + t0 * V, vb->d_out.get(), t1 - t0, row_mask, n_planes, s));
-          MLB_TRY(mlb_controllers_process_device(cb, cb->d_off.get() + t0 * G1, cb->d_ch.get(), vb->d_out.get(),
-                                                 MLB_VOICE_ROWS, n_planes, t1 - t0, s));
-          return graph_process(g, vb->d_out.get(), n_planes, out_host ? g->d_out.get() + t0 * row_floats : nullptr,
-                               mix_host ? g->d_mix.get() + t0 * n_out * MLB_BLOCK : nullptr, t1 - t0, s);
-        },
-        [&](int t0, int t1, cudaStream_t s)
-        {
-          return cudaMemcpyAsync(out_host + t0 * row_floats, g->d_out.get() + t0 * row_floats,
-                                 (t1 - t0) * row_floats * 4, cudaMemcpyDeviceToHost, s);
-        }));
-    if (mix_host) MLB_TRY(mlb_graph_mix_wait(g, g->stream.get()));
-    if (mix_host)
-      CU_CHECK(cudaMemcpyAsync(mix_host, g->d_mix.get(), T * n_out * MLB_BLOCK * 4, cudaMemcpyDeviceToHost, g->stream.get()));
-    return MLB_OK;
-  }();
-  return drain(rc, {g->s_h2d.get(), g->stream.get(), g->s_d2h.get()});
+  MLB_TRY(check_offsets(ctrl_offsets_host, cb->G, n_changes, n_blocks, "change", "changes"));
+  c.vb = vb, c.g = g, c.n_blocks = n_blocks, c.records = events_host, c.out = out_host, c.mix = mix_host;
+  c.cb = cb, c.ctrl_offsets = ctrl_offsets_host, c.ctrl_changes = ctrl_changes_host, c.n_changes = n_changes;
+  return c.run();
 }
 
 // ------------------------------------------------------------------------------------------
@@ -3099,20 +3038,6 @@ extern "C" int mlb_process_time_process_device(mlb_process_time* pt, const int32
   return MLB_OK;
 }
 
-// offsets [T][G + 1] must index transports of n_transports entries, non-decreasing within each block
-static int process_time_check_offsets(const mlb_process_time* pt, const int32_t* offsets, int n_transports, int n_blocks)
-{
-  for (int t = 0; t < n_blocks; ++t)
-  {
-    const int32_t* o = offsets + (size_t)t * (pt->G + 1);
-    for (int g = 0; g < pt->G; ++g)
-      if (o[g] < 0 || o[g] > o[g + 1] || o[g + 1] > n_transports)
-        return fail(MLB_ERR_INVALID, "block %d, instrument %d: transport range [%d, %d) is not within the %d updates", t,
-                    g, o[g], o[g + 1], n_transports);
-  }
-  return MLB_OK;
-}
-
 extern "C" int mlb_process_time_process_host(mlb_process_time* pt, const int32_t* offsets_host,
                                              const mlb_transport* transports_host, int n_transports, float* out_host,
                                              int plane0, int n_planes, int n_blocks)
@@ -3121,7 +3046,7 @@ extern "C" int mlb_process_time_process_host(mlb_process_time* pt, const int32_t
     return fail(MLB_ERR_INVALID, "null argument");
   if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive (got %d)", n_blocks);
   if (n_transports < 0) return fail(MLB_ERR_INVALID, "n_transports must not be negative (got %d)", n_transports);
-  MLB_TRY(process_time_check_offsets(pt, offsets_host, n_transports, n_blocks));
+  MLB_TRY(check_offsets(offsets_host, pt->G, n_transports, n_blocks, "transport", "updates"));
   if (plane0 < 0 || n_planes <= plane0)
     return fail(MLB_ERR_INVALID, "beat-phase plane %d is not within the %d output planes", plane0, n_planes);
   const size_t T = (size_t)n_blocks, N = pt->V ? pt->V : pt->G;
@@ -3290,23 +3215,17 @@ static int routers_check(const mlb_routers* r, const int32_t* offsets, const mlb
   if (n_events < 0) return fail(MLB_ERR_INVALID, "n_events must not be negative (got %d)", n_events);
   if (n_events > 0 && !events) return fail(MLB_ERR_INVALID, "null events");
   int64_t n = 0;
-  for (int t = 0; t < n_blocks; ++t)
+  MLB_TRY(check_offsets(offsets, r->G, n_events, n_blocks, "event", "events", [&](int t, int g, int i0, int i1) -> int
   {
-    const int32_t* o = offsets + (size_t)t * (r->G + 1);
-    for (int g = 0; g < r->G; ++g)
+    for (int i = i0; i < i1; ++i)
     {
-      if (o[g] < 0 || o[g] > o[g + 1] || o[g + 1] > n_events)
-        return fail(MLB_ERR_INVALID, "block %d, instrument %d: event range [%d, %d) is not within the %d events", t, g,
-                    o[g], o[g + 1], n_events);
-      for (int i = o[g]; i < o[g + 1]; ++i)
-      {
-        if (events[i].time < 0 || events[i].time >= MLB_BLOCK)
-          return fail(MLB_ERR_INVALID, "block %d, instrument %d, event %d: time %d is not a frame of the vector (0..%d)",
-                      t, g, i, (int)events[i].time, MLB_BLOCK - 1);
-        n += router_writes_controller(events[i].type, r->protocol);
-      }
+      if (events[i].time < 0 || events[i].time >= MLB_BLOCK)
+        return fail(MLB_ERR_INVALID, "block %d, instrument %d, event %d: time %d is not a frame of the vector (0..%d)", t,
+                    g, i, (int)events[i].time, MLB_BLOCK - 1);
+      n += router_writes_controller(events[i].type, r->protocol);
     }
-  }
+    return MLB_OK;
+  }));
   if (n > 0x7FFFFFFF) return fail(MLB_ERR_INVALID, "%lld controller writes exceed one call", (long long)n);
   *n_changes = (int)n;
   return MLB_OK;
@@ -3355,9 +3274,7 @@ extern "C" int mlb_routers_process_host(mlb_routers* r, const int32_t* offsets_h
   return drain(rc, {s});
 }
 
-// Contract E from raw events: per time chunk on host_pipeline, the chunk's offsets go up on s_h2d (all events and
-// transport updates with the first chunk); K12, the voice kernel, K11 (if given), K13 (if given), the graph and the bus
-// sum (if given) run on the graph's stream into one chunk of device buffers; output or bus rows come down on s_d2h.
+// The checks of contract E from raw events (the routed and context entry points), then the driver.
 static int synth_routed(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb, mlb_process_time* pt, mlb_graph* g,
                         mlb_buses* b, const int32_t* offsets_host, const mlb_event* events_host, int n_events,
                         const int32_t* time_offsets_host, const mlb_transport* transports_host, int n_transports,
@@ -3366,10 +3283,9 @@ static int synth_routed(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb, mlb
   if (!r || !offsets_host) return fail(MLB_ERR_INVALID, "null argument");
   if (b ? (!bus_host || out_host || mix_host) : bus_host != nullptr)
     return fail(MLB_ERR_INVALID, "bus rows come with a bus layout, and then alone (out and mix must be null)");
-  const int phase_plane = MLB_VOICE_ROWS + (cb ? cb->C : 0);
-  const int n_planes = phase_plane + (pt ? 1 : 0);
-  unsigned row_mask;
-  MLB_TRY(synth_check(vb, g, offsets_host, n_blocks, out_host || mix_host || bus_host, &row_mask, n_planes,
+  SynthCall c;
+  c.n_planes = MLB_VOICE_ROWS + (cb ? cb->C : 0) + (pt ? 1 : 0);
+  MLB_TRY(synth_check(vb, g, offsets_host, n_blocks, out_host || mix_host || bus_host, &c.row_mask, c.n_planes,
                       pt != nullptr));
   if (r->V != g->V) return fail(MLB_ERR_INVALID, "router bank writes %d voices, graph has %d", r->V, g->V);
   if ((r->protocol == 0) != ((vb->flags & MLB_VOICES_MIDI) != 0))
@@ -3395,26 +3311,64 @@ static int synth_routed(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb, mlb
     return fail(MLB_ERR_INVALID, "%d transport updates at %p", n_transports, (const void*)transports_host);
   int n_changes = 0;
   MLB_TRY(routers_check(r, offsets_host, events_host, n_events, n_blocks, &n_changes));
-  if (pt) MLB_TRY(process_time_check_offsets(pt, time_offsets_host, n_transports, n_blocks));
+  if (pt) MLB_TRY(check_offsets(time_offsets_host, pt->G, n_transports, n_blocks, "transport", "updates"));
+  c.vb = vb, c.g = g, c.n_blocks = n_blocks, c.out = out_host, c.mix = mix_host, c.b = b, c.bus = bus_host;
+  c.r = r, c.offsets = offsets_host, c.events = events_host, c.n_events = n_events, c.n_changes = n_changes, c.cb = cb;
+  c.pt = pt, c.time_offsets = time_offsets_host, c.transports = transports_host, c.n_transports = n_transports;
+  return c.run();
+}
+
+// Rows [t0, t1) of a [T][G + 1] offset table into the same rows of dev_off, and with the first chunk the whole list of
+// n items it indexes into dev_items.
+template <class Item>
+static cudaError_t upload_list_chunk(int32_t* dev_off, const int32_t* off, size_t G1, Item* dev_items, const Item* items,
+                                     int n, int t0, int t1, cudaStream_t s)
+{
+  cudaError_t e = cudaSuccess;
+  if (t0 == 0 && n) e = cudaMemcpyAsync(dev_items, items, n * sizeof(Item), cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess)
+    e = cudaMemcpyAsync(dev_off + t0 * G1, off + t0 * G1, (t1 - t0) * G1 * 4, cudaMemcpyHostToDevice, s);
+  return e;
+}
+
+// The contract-E driver, on host_pipeline over time chunks of Tc blocks: the chunk's records or raw-event offsets, and
+// the offsets of the host's controller changes and transport updates, go up on s_h2d (every list they index with the
+// first chunk); K12, the voice kernel, K11, K13, the graph and the bus sum run on the graph's stream; out or bus rows
+// come down on s_d2h, the mix bus after the last chunk.
+// Data the host uploads per chunk lands at the chunk's own rows of a buffer sized for the whole call (the records in
+// vb->d_ev, every offset table): s_h2d does not wait for the previous chunk's kernels, so an upload into one chunk's
+// buffer at offset 0 would overwrite what they may still be reading.  Only what the device writes on the graph's
+// stream, the router's records (vb->d_ev) and change offsets (r->d_coff), reuses one chunk's buffer at offset 0.
+int SynthCall::run() const
+{
   MLB_TRY(ensure_init());
-  const size_t V = (size_t)g->V, T = (size_t)n_blocks, n_out = g->outs.size(), G1 = (size_t)r->G + 1;
+  const size_t V = (size_t)g->V, T = (size_t)n_blocks, n_out = g->outs.size();
+  const size_t G1 = (size_t)(r ? r->G : cb ? cb->G : 0) + 1;  // pt->G is r->G
   const int Tc = synth_chunk_blocks(g, n_blocks, n_planes);
-  if (out_host) MLB_TRY(g->d_out.ensure(T * n_out * V * MLB_BLOCK * 4, "staging"));
+  if (out) MLB_TRY(g->d_out.ensure(T * n_out * V * MLB_BLOCK * 4, "staging"));
   if (b) MLB_TRY(g->d_out.ensure((size_t)Tc * n_out * V * MLB_BLOCK * 4, "staging"));
   if (b) MLB_TRY(b->d_out.ensure(T * n_out * b->G * MLB_BLOCK * 4, "staging"));
-  if (mix_host) MLB_TRY(g->d_mix.ensure(T * n_out * MLB_BLOCK * 4, "staging"));
-  MLB_TRY(r->d_off.ensure(T * G1 * 4, "staging"));
-  MLB_TRY(r->d_coff.ensure((size_t)Tc * G1 * 4, "staging"));
-  MLB_TRY(r->d_ev.ensure(std::max(n_events, 1) * sizeof(mlb_event), "staging"));
-  MLB_TRY(r->d_ch.ensure(std::max(n_changes, 1) * sizeof(mlb_controller_change), "staging"));
-  MLB_TRY(vb->d_ev.ensure((size_t)Tc * V * sizeof(mlb_voice_events), "staging"));
+  if (mix) MLB_TRY(g->d_mix.ensure(T * n_out * MLB_BLOCK * 4, "staging"));
+  if (r)
+  {
+    MLB_TRY(r->d_off.ensure(T * G1 * 4, "staging"));
+    MLB_TRY(r->d_coff.ensure((size_t)Tc * G1 * 4, "staging"));
+    MLB_TRY(r->d_ev.ensure(std::max(n_events, 1) * sizeof(mlb_event), "staging"));
+    MLB_TRY(r->d_ch.ensure(std::max(n_changes, 1) * sizeof(mlb_controller_change), "staging"));
+  }
+  MLB_TRY(vb->d_ev.ensure((r ? (size_t)Tc : T) * V * sizeof(mlb_voice_events), "staging"));
   MLB_TRY(vb->d_out.ensure((size_t)Tc * n_planes * V * MLB_BLOCK * 4, "staging"));
+  if (cb && !r)
+  {
+    MLB_TRY(cb->d_off.ensure(T * G1 * 4, "staging"));
+    if (n_changes) MLB_TRY(cb->d_ch.ensure((size_t)n_changes * sizeof(mlb_controller_change), "staging"));
+  }
   if (pt) MLB_TRY(pt->d_off.ensure(T * G1 * 4, "staging"));
   if (pt) MLB_TRY(pt->d_tr.ensure(std::max(n_transports, 1) * sizeof(mlb_transport), "staging"));
   const size_t row_floats = n_out * V * MLB_BLOCK;             // output rows per block
   const size_t bus_floats = b ? n_out * b->G * MLB_BLOCK : 0;  // bus rows per block
   float* down_dev = b ? b->d_out.get() : g->d_out.get();
-  float* down_host = b ? bus_host : out_host;
+  float* down_host = b ? bus : out;
   const size_t down_floats = b ? bus_floats : row_floats;
   const int rc = [&]() -> int
   {
@@ -3422,47 +3376,45 @@ static int synth_routed(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb, mlb
         g, n_blocks, Tc, true, down_host != nullptr,
         [&](int t0, int t1, cudaStream_t s)
         {
-          cudaError_t e = cudaSuccess;
-          if (t0 == 0 && n_events)
-            e = cudaMemcpyAsync(r->d_ev.get(), events_host, n_events * sizeof(mlb_event), cudaMemcpyHostToDevice, s);
-          if (e == cudaSuccess)
-            e = cudaMemcpyAsync(r->d_off.get() + t0 * G1, offsets_host + t0 * G1, (t1 - t0) * G1 * 4,
-                                cudaMemcpyHostToDevice, s);
-          if (e == cudaSuccess && pt && t0 == 0 && n_transports)
-            e = cudaMemcpyAsync(pt->d_tr.get(), transports_host, n_transports * sizeof(mlb_transport),
-                                cudaMemcpyHostToDevice, s);
+          cudaError_t e =
+              r ? upload_list_chunk(r->d_off.get(), offsets, G1, r->d_ev.get(), events, n_events, t0, t1, s)
+                : cudaMemcpyAsync(vb->d_ev.get() + t0 * V, records + t0 * V, (t1 - t0) * V * sizeof(mlb_voice_events),
+                                  cudaMemcpyHostToDevice, s);
+          if (e == cudaSuccess && cb && !r)
+            e = upload_list_chunk(cb->d_off.get(), ctrl_offsets, G1, cb->d_ch.get(), ctrl_changes, n_changes, t0, t1, s);
           if (e == cudaSuccess && pt)
-            e = cudaMemcpyAsync(pt->d_off.get() + t0 * G1, time_offsets_host + t0 * G1, (t1 - t0) * G1 * 4,
-                                cudaMemcpyHostToDevice, s);
+            e = upload_list_chunk(pt->d_off.get(), time_offsets, G1, pt->d_tr.get(), transports, n_transports, t0, t1, s);
           return e;
         },
         [&](int t0, int t1, cudaStream_t s) -> int
         {
-          MLB_TRY(mlb_routers_process_device(r, r->d_off.get() + t0 * G1, r->d_ev.get(), vb->d_ev.get(), r->d_coff.get(),
-                                             r->d_ch.get(), t1 - t0, s));
-          MLB_TRY(voices_launch(vb, vb->d_ev.get(), vb->d_out.get(), t1 - t0, row_mask, n_planes, s));
+          if (r)
+            MLB_TRY(mlb_routers_process_device(r, r->d_off.get() + t0 * G1, r->d_ev.get(), vb->d_ev.get(),
+                                               r->d_coff.get(), r->d_ch.get(), t1 - t0, s));
+          MLB_TRY(voices_launch(vb, vb->d_ev.get() + (r ? 0 : t0 * V), vb->d_out.get(), t1 - t0, row_mask, n_planes, s));
           if (cb)
-            MLB_TRY(mlb_controllers_process_device(cb, r->d_coff.get(), r->d_ch.get(), vb->d_out.get(), MLB_VOICE_ROWS,
+            MLB_TRY(mlb_controllers_process_device(cb, r ? r->d_coff.get() : cb->d_off.get() + t0 * G1,
+                                                   r ? r->d_ch.get() : cb->d_ch.get(), vb->d_out.get(), MLB_VOICE_ROWS,
                                                    n_planes, t1 - t0, s));
           if (pt)
             MLB_TRY(mlb_process_time_process_device(pt, pt->d_off.get() + t0 * G1, pt->d_tr.get(), vb->d_out.get(),
-                                                    phase_plane, n_planes, t1 - t0, s));
+                                                    n_planes - 1, n_planes, t1 - t0, s));
           if (b)
           {
             MLB_TRY(graph_process(g, vb->d_out.get(), n_planes, g->d_out.get(), nullptr, t1 - t0, s));
             return mlb_buses_sum_device(b, g->d_out.get(), b->d_out.get() + t0 * bus_floats, (int)n_out, t1 - t0, s);
           }
-          return graph_process(g, vb->d_out.get(), n_planes, out_host ? g->d_out.get() + t0 * row_floats : nullptr,
-                               mix_host ? g->d_mix.get() + t0 * n_out * MLB_BLOCK : nullptr, t1 - t0, s);
+          return graph_process(g, vb->d_out.get(), n_planes, out ? g->d_out.get() + t0 * row_floats : nullptr,
+                               mix ? g->d_mix.get() + t0 * n_out * MLB_BLOCK : nullptr, t1 - t0, s);
         },
         [&](int t0, int t1, cudaStream_t s)
         {
           return cudaMemcpyAsync(down_host + t0 * down_floats, down_dev + t0 * down_floats,
                                  (t1 - t0) * down_floats * 4, cudaMemcpyDeviceToHost, s);
         }));
-    if (mix_host) MLB_TRY(mlb_graph_mix_wait(g, g->stream.get()));
-    if (mix_host)
-      CU_CHECK(cudaMemcpyAsync(mix_host, g->d_mix.get(), T * n_out * MLB_BLOCK * 4, cudaMemcpyDeviceToHost, g->stream.get()));
+    if (mix) MLB_TRY(mlb_graph_mix_wait(g, g->stream.get()));
+    if (mix)
+      CU_CHECK(cudaMemcpyAsync(mix, g->d_mix.get(), T * n_out * MLB_BLOCK * 4, cudaMemcpyDeviceToHost, g->stream.get()));
     return MLB_OK;
   }();
   return drain(rc, {g->s_h2d.get(), g->stream.get(), g->s_d2h.get()});
