@@ -198,6 +198,23 @@ def _ptr(a) -> Optional[int]:
     raise TypeError(type(a))
 
 
+def _offset_table(name: str, offsets, n_instruments: int):
+    """(offsets as a C-contiguous int32 [T][n_instruments + 1] array, T)."""
+    off = np.ascontiguousarray(offsets, np.int32)
+    if off.ndim != 2 or off.shape[1] != n_instruments + 1:
+        raise ValueError(f"{name}: offsets must be [T][{n_instruments + 1}], got {off.shape}")
+    return off, int(off.shape[0])
+
+
+def _out_array(name: str, key: str, a, shape, new=np.empty) -> np.ndarray:
+    """`a`, or new(shape) if it is None: a C-contiguous float32 array of `shape`, which the library writes in place."""
+    if a is None:
+        a = new(shape, np.float32)
+    if not (isinstance(a, np.ndarray) and a.dtype == np.float32 and a.flags["C_CONTIGUOUS"] and a.shape == shape):
+        raise ValueError(f"{name}: `{key}` must be a C-contiguous float32 array of shape {shape}")
+    return a
+
+
 def device_count() -> int:
     return int(lib().mlb_device_count())
 
@@ -390,15 +407,10 @@ class VoiceGraph(_Handle):
         if s.n_in:
             assert inp is not None and inp.dtype == np.float32 and inp.flags["C_CONTIGUOUS"]
             assert inp.shape == (T, s.n_in, V, BLOCK), inp.shape
-        if want_out and out is None:
-            out = np.empty((T, s.n_out, V, BLOCK), np.float32)
-        if want_mix and mix is None:
-            mix = np.empty((T, s.n_out, BLOCK), np.float32)
-        for name, a, shape in (("out", out if want_out else None, (T, s.n_out, V, BLOCK)),
-                               ("mix", mix if want_mix else None, (T, s.n_out, BLOCK))):
-            if a is not None and not (isinstance(a, np.ndarray) and a.dtype == np.float32 and
-                                      a.flags["C_CONTIGUOUS"] and a.shape == shape):
-                raise ValueError(f"process_host: `{name}` must be a C-contiguous float32 array of shape {shape}")
+        if want_out:
+            out = _out_array("process_host", "out", out, (T, s.n_out, V, BLOCK))
+        if want_mix:
+            mix = _out_array("process_host", "mix", mix, (T, s.n_out, BLOCK))
         _check(lib().mlb_graph_process_host(self._h, _ptr(inp) if s.n_in else None,
                                             _ptr(out) if want_out else None,
                                             _ptr(mix) if want_mix else None, T))
@@ -417,22 +429,14 @@ class VoiceGraph(_Handle):
                 raise ValueError(f"{name}: `events` must be a C-contiguous [T][V] array of 72-byte records")
             T = int(events.shape[0])
         else:
-            offsets = np.ascontiguousarray(offsets, np.int32)
-            if offsets.ndim != 2 or offsets.shape[1] != n_instruments + 1:
-                raise ValueError(f"{name}: offsets must be [T][{n_instruments + 1}], got {offsets.shape}")
-            T = int(offsets.shape[0])
+            offsets, T = _offset_table(name, offsets, n_instruments)
         shape = (T, s.n_out, V, BLOCK)
         if buses is not None:
             shape, want_out, want_mix = (T, s.n_out, buses.n_buses, BLOCK), True, False
-        if want_out and out is None:
-            out = np.empty(shape, np.float32)
-        if want_mix and mix is None:
-            mix = np.empty((T, s.n_out, BLOCK), np.float32)
-        for key, a, shp in (("out", out if want_out else None, shape),
-                            ("mix", mix if want_mix else None, (T, s.n_out, BLOCK))):
-            if a is not None and not (isinstance(a, np.ndarray) and a.dtype == np.float32 and
-                                      a.flags["C_CONTIGUOUS"] and a.shape == shp):
-                raise ValueError(f"{name}: `{key}` must be a C-contiguous float32 array of shape {shp}")
+        if want_out:
+            out = _out_array(name, "out", out, shape)
+        if want_mix:
+            mix = _out_array(name, "mix", mix, (T, s.n_out, BLOCK))
         return T, offsets, out, mix
 
     def process_events_host(self, bank: "VoiceBank", events: np.ndarray, want_out: bool = True,
@@ -652,10 +656,36 @@ class Buses(_Handle):
                                           stream or None))
 
 
+class _ListBank(_Handle):
+    """What ControllerBank and ProcessTimeBank share: per block a CSR list, offsets [T][G + 1] into items, in; rows
+    [T][n_planes][N][64] out, N = G instrument rows or N = V voice rows after set_voice_map.  ``_prefix`` names the
+    library's functions of the bank."""
+
+    _prefix = ""
+    n_voices = 0  # V of the voice map; 0: instrument rows
+
+    def set_voice_map(self, voice_instrument) -> None:
+        """voice_instrument[V]: each voice's instrument or -1; None goes back to instrument rows."""
+        vm = None if voice_instrument is None else np.ascontiguousarray(voice_instrument, np.int32)
+        n = 0 if vm is None else int(vm.shape[0])
+        _check(getattr(lib(), self._prefix + "_set_voice_map")(self._h, _ptr(vm), n))
+        self.n_voices = n
+
+    def _process_host(self, offsets, items, dtype, out, plane0, n_planes) -> np.ndarray:
+        off, T = _offset_table("process_host", offsets, self.n_instruments)
+        it = np.ascontiguousarray(items, dtype)
+        P = int(n_planes)
+        out = _out_array("process_host", "out", out, (T, P, self.n_voices or self.n_instruments, BLOCK), np.zeros)
+        fn = getattr(lib(), self._prefix + "_process_host")
+        _check(fn(self._h, off.ctypes.data, it.ctypes.data if it.size else None, int(it.size), out.ctypes.data,
+                  int(plane0), P, T))
+        return out
+
+
 CONTROLLER_CHANGE_DTYPE = np.dtype([("controller", "<u2"), ("pad", "<u2"), ("value", "<f4")])  # mlb_controller_change
 
 
-class ControllerBank(_Handle):
+class ControllerBank(_ListBank):
     """G instruments x C requested MIDI controllers (mlb_controllers_*): the SmoothedControllers of one reference
     EventsToSignals per instrument (MLEventsToSignals.h:170-180), i.e. what AudioContext::getInputController(n)
     returns, bit for bit.  Input per block: a CSR change list, offsets [T][G + 1] into changes
@@ -664,6 +694,7 @@ class ControllerBank(_Handle):
     a voice of instrument -1 gets +0)."""
 
     _destroy = "mlb_controllers_destroy"
+    _prefix = "mlb_controllers"
 
     MIDI, MPE = 0, 1
     N_WORDS = 4  # state words: inputValue, target, vectorsRemaining, step
@@ -673,7 +704,7 @@ class ControllerBank(_Handle):
         if ctrl.ndim != 1:
             raise ValueError(f"ControllerBank: `controllers` must be a 1-D list of numbers, got shape {ctrl.shape}")
         self.n_instruments, self.controllers = int(n_instruments), [int(c) for c in ctrl]
-        self.n_controllers, self.protocol, self.n_voices = len(self.controllers), int(protocol), 0
+        self.n_controllers, self.protocol = len(self.controllers), int(protocol)
         h = ctypes.c_void_p()
         _check(lib().mlb_controllers_create(self.n_instruments, sample_rate, self.protocol, ctrl.ctypes.data,
                                             self.n_controllers, ctypes.byref(h)))
@@ -699,35 +730,12 @@ class ControllerBank(_Handle):
                              f"{r.shape}")
         _check(lib().mlb_controllers_set_state(self._h, w.ctypes.data, r.ctypes.data))
 
-    def set_voice_map(self, voice_instrument) -> None:
-        """voice_instrument[V]: each voice's instrument or -1; None goes back to instrument rows."""
-        if voice_instrument is None:
-            _check(lib().mlb_controllers_set_voice_map(self._h, None, 0))
-            self.n_voices = 0
-            return
-        vm = np.ascontiguousarray(voice_instrument, np.int32)
-        _check(lib().mlb_controllers_set_voice_map(self._h, vm.ctypes.data, int(vm.shape[0])))
-        self.n_voices = int(vm.shape[0])
-
     def process_host(self, offsets: np.ndarray, changes: np.ndarray, out: Optional[np.ndarray] = None,
                      plane0: int = 0, n_planes: Optional[int] = None) -> np.ndarray:
         """offsets [T][G + 1] int32, changes (CONTROLLER_CHANGE_DTYPE) -> out [T][n_planes][N][64]; planes outside
         [plane0, plane0 + C) of a given `out` are left as they are."""
-        off = np.ascontiguousarray(offsets, np.int32)
-        if off.ndim != 2 or off.shape[1] != self.n_instruments + 1:
-            raise ValueError(f"process_host: offsets must be [T][{self.n_instruments + 1}], got {off.shape}")
-        ch = np.ascontiguousarray(changes, CONTROLLER_CHANGE_DTYPE)
-        T = int(off.shape[0])
-        P = self.n_controllers if n_planes is None else int(n_planes)
-        shape = (T, P, self.n_voices or self.n_instruments, BLOCK)
-        if out is None:
-            out = np.zeros(shape, np.float32)
-        if not (isinstance(out, np.ndarray) and out.dtype == np.float32 and out.flags["C_CONTIGUOUS"] and
-                out.shape == shape):
-            raise ValueError(f"process_host: `out` must be a C-contiguous float32 array of shape {shape}")
-        _check(lib().mlb_controllers_process_host(self._h, off.ctypes.data, ch.ctypes.data if ch.size else None,
-                                                  int(ch.size), out.ctypes.data, int(plane0), P, T))
-        return out
+        P = self.n_controllers if n_planes is None else n_planes
+        return self._process_host(offsets, changes, CONTROLLER_CHANGE_DTYPE, out, plane0, P)
 
     def process_device(self, offsets, changes, out, n_blocks: int, plane0: int = 0, n_planes: Optional[int] = None,
                        stream: int = 0) -> None:
@@ -742,7 +750,7 @@ TRANSPORT_DTYPE = np.dtype([("ppq_pos", "<f8"), ("bpm", "<f8"), ("sample_rate", 
                             ("pad", "<i4")])  # mlb_transport
 
 
-class ProcessTimeBank(_Handle):
+class ProcessTimeBank(_ListBank):
     """G host-transport clocks (mlb_process_time_*): the AudioContext::ProcessTime of one reference AudioContext per
     instrument, i.e. what AudioContext::getBeatPhase() returns, bit for bit.  Input per block: a CSR list of transport
     updates, offsets [T][G + 1] into transports (TRANSPORT_DTYPE), each applied in order as
@@ -750,13 +758,14 @@ class ProcessTimeBank(_Handle):
     or N = V after set_voice_map (every voice gets its instrument's row, a voice of instrument -1 gets +0)."""
 
     _destroy = "mlb_process_time_destroy"
+    _prefix = "mlb_process_time"
 
     N_WORDS = 10  # omega_, dpdt_, ppqPos1_, ppqPhase1_, playing1_, active1_, samplesSincePreviousTime_,
     #               samplesSinceStart, bpm, sampleRate
 
     def __init__(self, n_instruments: int, sample_rate: float = 48000.0):
         """sample_rate: whole hertz, as AudioContext(nIn, nOut, int rate) takes it (a fractional rate is refused)."""
-        self.n_instruments, self.n_voices = int(n_instruments), 0
+        self.n_instruments = int(n_instruments)
         h = ctypes.c_void_p()
         _check(lib().mlb_process_time_create(self.n_instruments, float(sample_rate), ctypes.byref(h)))
         self._h = h
@@ -777,34 +786,11 @@ class ProcessTimeBank(_Handle):
             raise ValueError(f"set_state: words must be [10][{self.n_instruments}], got {w.shape}")
         _check(lib().mlb_process_time_set_state(self._h, w.ctypes.data))
 
-    def set_voice_map(self, voice_instrument) -> None:
-        """voice_instrument[V]: each voice's instrument or -1; None goes back to instrument rows."""
-        if voice_instrument is None:
-            _check(lib().mlb_process_time_set_voice_map(self._h, None, 0))
-            self.n_voices = 0
-            return
-        vm = np.ascontiguousarray(voice_instrument, np.int32)
-        _check(lib().mlb_process_time_set_voice_map(self._h, vm.ctypes.data, int(vm.shape[0])))
-        self.n_voices = int(vm.shape[0])
-
     def process_host(self, offsets: np.ndarray, transports: np.ndarray, out: Optional[np.ndarray] = None,
                      plane0: int = 0, n_planes: int = 1) -> np.ndarray:
         """offsets [T][G + 1] int32, transports (TRANSPORT_DTYPE) -> out [T][n_planes][N][64]; planes other than
         plane0 of a given `out` are left as they are."""
-        off = np.ascontiguousarray(offsets, np.int32)
-        if off.ndim != 2 or off.shape[1] != self.n_instruments + 1:
-            raise ValueError(f"process_host: offsets must be [T][{self.n_instruments + 1}], got {off.shape}")
-        tr = np.ascontiguousarray(transports, TRANSPORT_DTYPE)
-        T = int(off.shape[0])
-        shape = (T, int(n_planes), self.n_voices or self.n_instruments, BLOCK)
-        if out is None:
-            out = np.zeros(shape, np.float32)
-        if not (isinstance(out, np.ndarray) and out.dtype == np.float32 and out.flags["C_CONTIGUOUS"] and
-                out.shape == shape):
-            raise ValueError(f"process_host: `out` must be a C-contiguous float32 array of shape {shape}")
-        _check(lib().mlb_process_time_process_host(self._h, off.ctypes.data, tr.ctypes.data if tr.size else None,
-                                                   int(tr.size), out.ctypes.data, int(plane0), int(n_planes), T))
-        return out
+        return self._process_host(offsets, transports, TRANSPORT_DTYPE, out, plane0, n_planes)
 
     def process_device(self, offsets, transports, out, n_blocks: int, plane0: int = 0, n_planes: int = 1,
                        stream: int = 0) -> None:
@@ -986,11 +972,8 @@ class RouterBank(_Handle):
         """-> (records [T][V] of workloads.VOICE_EVENTS_DTYPE, change_offsets [T][G + 1] int32, changes of
         CONTROLLER_CHANGE_DTYPE)."""
         from .workloads import VOICE_EVENTS_DTYPE
-        off = np.ascontiguousarray(offsets, np.int32)
-        if off.ndim != 2 or off.shape[1] != self.n_instruments + 1:
-            raise ValueError(f"process_host: offsets must be [T][{self.n_instruments + 1}], got {off.shape}")
+        off, T = _offset_table("process_host", offsets, self.n_instruments)
         ev = np.ascontiguousarray(events, EVENT_DTYPE)
-        T = int(off.shape[0])
         rec = np.empty((T, self.n_voices), VOICE_EVENTS_DTYPE)
         coff = np.empty((T, self.n_instruments + 1), np.int32)
         n = ctypes.c_int(0)

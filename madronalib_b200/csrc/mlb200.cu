@@ -2685,21 +2685,79 @@ extern "C" int mlb_synth_process_buses_host(mlb_voices* vb, mlb_graph* g, mlb_bu
 // ------------------------------------------------------------------------------------------
 // Smoothed MIDI controllers (K11, controller_kernel.cuh)
 
-struct mlb_controllers
+// The base of the controller and process-time banks: per block a CSR list, offsets [T][G + 1] into items, in; the
+// rows of G instruments or, after set_voice_map, of V mapped voices out, in planes [plane0, plane0 + n) of an output.
+struct ListBank
 {
-  // declared first, so released last: the buffers below are freed first, and cudaFree waits for the device
+  // declared first, so released last: all buffers (a bank's own too) are freed first, and cudaFree waits for the device
   LiveCount live;
   Stream stream;
-  int G = 0, C = 0, protocol = 0;
-  int V = 0;  // voices of the voice map; 0: instrument rows
+  int G = 0;
+  int V = 0;               // voices of the voice map; 0: instrument rows
+  DevBuf<int32_t> d_vmap;  // [G + 2] offsets, then [V] voices grouped by instrument, the unmapped ones last
+  DevBuf<int32_t> d_off;   // staging of the host entry points
+  DevBuf<float> d_out;
+};
+
+// The kernel arguments CtrlArgs and PtArgs share: the list's offsets, the output and the rows the bank writes.
+template <class Args>
+static void list_bank_args(const ListBank& b, Args& a, const int32_t* offsets, float* out, int plane0, int n_planes,
+                           int n_blocks)
+{
+  a.offsets = offsets, a.out = out;
+  a.vmap_off = b.V ? b.d_vmap.get() : nullptr;
+  a.vmap_voice = b.V ? b.d_vmap.get() + b.G + 2 : nullptr;
+  a.G = b.G, a.N = b.V ? b.V : b.G, a.T = n_blocks;
+  a.plane0 = plane0, a.n_planes = n_planes;
+  a.n_gblk = (b.G + 31) / 32;
+}
+
+// Rows [t0, t1) of a [T][G + 1] offset table into the same rows of dev_off, and with the first chunk the whole list of
+// n items it indexes into dev_items.
+template <class Item>
+static cudaError_t upload_list_chunk(int32_t* dev_off, const int32_t* off, size_t G1, Item* dev_items, const Item* items,
+                                     int n, int t0, int t1, cudaStream_t s)
+{
+  cudaError_t e = cudaSuccess;
+  if (t0 == 0 && n) e = cudaMemcpyAsync(dev_items, items, n * sizeof(Item), cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess)
+    e = cudaMemcpyAsync(dev_off + t0 * G1, off + t0 * G1, (t1 - t0) * G1 * 4, cudaMemcpyHostToDevice, s);
+  return e;
+}
+
+// A bank's host entry once its arguments are checked: the offsets and all n_items items go up, its device entry runs,
+// and only planes [plane0, plane0 + n) come down: the caller's other planes stay as they were.
+template <class Bank, class Item>
+static int list_bank_host(Bank* b, int (*device)(Bank*, const int32_t*, const Item*, float*, int, int, int, void*),
+                          DevBuf<Item>& d_items, const int32_t* offsets_host, const Item* items_host, int n_items,
+                          float* out_host, int plane0, int n, int n_planes, int n_blocks)
+{
+  const size_t T = (size_t)n_blocks, N = b->V ? b->V : b->G, G1 = (size_t)b->G + 1;
+  MLB_TRY(b->d_off.ensure(T * G1 * 4, "staging"));
+  if (n_items) MLB_TRY(d_items.ensure((size_t)n_items * sizeof(Item), "staging"));
+  MLB_TRY(b->d_out.ensure(T * n_planes * N * MLB_BLOCK * 4, "staging"));
+  cudaStream_t s = b->stream.get();
+  const int rc = [&]() -> int
+  {
+    CU_CHECK(upload_list_chunk(b->d_off.get(), offsets_host, G1, d_items.get(), items_host, n_items, 0, n_blocks, s));
+    MLB_TRY(device(b, b->d_off.get(), d_items.get(), b->d_out.get(), plane0, n_planes, n_blocks, s));
+    const size_t plane = N * MLB_BLOCK * 4, pitch = (size_t)n_planes * plane;
+    CU_CHECK(cudaMemcpy2DAsync(reinterpret_cast<char*>(out_host) + plane0 * plane, pitch,
+                               reinterpret_cast<const char*>(b->d_out.get()) + plane0 * plane, pitch, n * plane, T,
+                               cudaMemcpyDeviceToHost, s));
+    return MLB_OK;
+  }();
+  return drain(rc, {s});
+}
+
+struct mlb_controllers : ListBank
+{
+  int C = 0, protocol = 0;
   float per_f = 0.f, dy = 0.f;
   DevBuf<int32_t> d_ctrl;   // [C] controller numbers
   DevBuf<uint32_t> d_state; // [CS_COUNT][C][G]
   DevBuf<float> d_rows;     // [C][G][64]
-  DevBuf<int32_t> d_vmap;   // [G + 2] offsets, then [V] voices grouped by instrument, the unmapped ones last
-  DevBuf<int32_t> d_off;    // staging of the host entry points
-  DevBuf<mlb_controller_change> d_ch;
-  DevBuf<float> d_out;
+  DevBuf<mlb_controller_change> d_ch;  // staging of the host entry points
 };
 
 extern "C" int mlb_controllers_destroy(mlb_controllers* cb)
@@ -2822,24 +2880,25 @@ extern "C" int mlb_controllers_set_voice_map(mlb_controllers* cb, const int32_t*
   return upload_voice_map(cb->G, voice_instrument, n_voices, cb->d_vmap, &cb->V);
 }
 
+static int controller_planes_check(const mlb_controllers* cb, int plane0, int n_planes)
+{
+  return plane0 < 0 || n_planes < plane0 + cb->C
+             ? fail(MLB_ERR_INVALID, "planes [%d, %d) of the %d controllers are not within the %d output planes",
+                    plane0, plane0 + cb->C, cb->C, n_planes)
+             : MLB_OK;
+}
+
 extern "C" int mlb_controllers_process_device(mlb_controllers* cb, const int32_t* offsets_dev,
                                               const mlb_controller_change* changes_dev, float* out_dev, int plane0,
                                               int n_planes, int n_blocks, void* stream)
 {
   if (!cb || !offsets_dev || !out_dev) return fail(MLB_ERR_INVALID, "null argument");
   if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive (got %d)", n_blocks);
-  if (plane0 < 0 || n_planes < plane0 + cb->C)
-    return fail(MLB_ERR_INVALID, "planes [%d, %d) of the %d controllers are not within the %d output planes", plane0,
-                plane0 + cb->C, cb->C, n_planes);
+  MLB_TRY(controller_planes_check(cb, plane0, n_planes));
   CtrlArgs a;
-  a.offsets = offsets_dev, a.changes = changes_dev, a.ctrl = cb->d_ctrl.get();
-  a.state = cb->d_state.get(), a.rows = cb->d_rows.get(), a.out = out_dev;
-  a.vmap_off = cb->V ? cb->d_vmap.get() : nullptr;
-  a.vmap_voice = cb->V ? cb->d_vmap.get() + cb->G + 2 : nullptr;
-  a.G = cb->G, a.C = cb->C, a.N = cb->V ? cb->V : cb->G, a.T = n_blocks;
-  a.plane0 = plane0, a.n_planes = n_planes;
-  a.n_gblk = (cb->G + 31) / 32;
-  a.per_f = cb->per_f, a.dy = cb->dy;
+  list_bank_args(*cb, a, offsets_dev, out_dev, plane0, n_planes, n_blocks);
+  a.changes = changes_dev, a.ctrl = cb->d_ctrl.get(), a.state = cb->d_state.get(), a.rows = cb->d_rows.get();
+  a.C = cb->C, a.per_f = cb->per_f, a.dy = cb->dy;
   const long long n_warps = (long long)a.C * a.n_gblk;
   controller_bank_kernel<<<(unsigned)((n_warps + kCtrlWarps - 1) / kCtrlWarps), 32 * kCtrlWarps, 0,
                            (cudaStream_t)stream>>>(a);
@@ -2882,30 +2941,9 @@ extern "C" int mlb_controllers_process_host(mlb_controllers* cb, const int32_t* 
   if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive (got %d)", n_blocks);
   if (n_changes < 0) return fail(MLB_ERR_INVALID, "n_changes must not be negative (got %d)", n_changes);
   MLB_TRY(check_offsets(offsets_host, cb->G, n_changes, n_blocks, "change", "changes"));
-  if (plane0 < 0 || n_planes < plane0 + cb->C)
-    return fail(MLB_ERR_INVALID, "planes [%d, %d) of the %d controllers are not within the %d output planes", plane0,
-                plane0 + cb->C, cb->C, n_planes);
-  const size_t T = (size_t)n_blocks, N = cb->V ? cb->V : cb->G;
-  const size_t off_bytes = T * (cb->G + 1) * 4, ch_bytes = (size_t)n_changes * sizeof(mlb_controller_change);
-  const size_t out_bytes = T * n_planes * N * MLB_BLOCK * 4;
-  MLB_TRY(cb->d_off.ensure(off_bytes, "staging"));
-  if (n_changes) MLB_TRY(cb->d_ch.ensure(ch_bytes, "staging"));
-  MLB_TRY(cb->d_out.ensure(out_bytes, "staging"));
-  cudaStream_t s = cb->stream.get();
-  const int rc = [&]() -> int
-  {
-    CU_CHECK(cudaMemcpyAsync(cb->d_off.get(), offsets_host, off_bytes, cudaMemcpyHostToDevice, s));
-    if (n_changes) CU_CHECK(cudaMemcpyAsync(cb->d_ch.get(), changes_host, ch_bytes, cudaMemcpyHostToDevice, s));
-    MLB_TRY(mlb_controllers_process_device(cb, cb->d_off.get(), cb->d_ch.get(), cb->d_out.get(), plane0, n_planes,
-                                           n_blocks, s));
-    // only the controller planes come down: the caller's other planes stay as they were
-    const size_t plane = N * MLB_BLOCK * 4, pitch = (size_t)n_planes * plane;
-    CU_CHECK(cudaMemcpy2DAsync(reinterpret_cast<char*>(out_host) + plane0 * plane, pitch,
-                               reinterpret_cast<const char*>(cb->d_out.get()) + plane0 * plane, pitch, cb->C * plane, T,
-                               cudaMemcpyDeviceToHost, s));
-    return MLB_OK;
-  }();
-  return drain(rc, {s});
+  MLB_TRY(controller_planes_check(cb, plane0, n_planes));
+  return list_bank_host(cb, mlb_controllers_process_device, cb->d_ch, offsets_host, changes_host, n_changes, out_host,
+                        plane0, cb->C, n_planes, n_blocks);
 }
 
 // Contract E with controller planes: the graph's input per block is the 8 Voice rows, then the C controller rows
@@ -2937,18 +2975,10 @@ extern "C" int mlb_synth_process_controllers_host(mlb_voices* vb, mlb_controller
 // ------------------------------------------------------------------------------------------
 // The host-transport beat phase of G instruments (K13, process_time_kernel.cuh)
 
-struct mlb_process_time
+struct mlb_process_time : ListBank
 {
-  // declared first, so released last: the buffers below are freed first, and cudaFree waits for the device
-  LiveCount live;
-  Stream stream;
-  int G = 0;
-  int V = 0;                 // voices of the voice map; 0: instrument rows
-  DevBuf<uint64_t> d_state;  // [MLB_PT_WORDS][G]
-  DevBuf<int32_t> d_vmap;    // upload_voice_map's table
-  DevBuf<int32_t> d_off;     // staging of the host entry points
-  DevBuf<mlb_transport> d_tr;
-  DevBuf<float> d_out;
+  DevBuf<uint64_t> d_state;    // [MLB_PT_WORDS][G]
+  DevBuf<mlb_transport> d_tr;  // staging of the host entry points
 };
 
 extern "C" int mlb_process_time_destroy(mlb_process_time* pt)
@@ -3017,21 +3047,23 @@ extern "C" int mlb_process_time_set_voice_map(mlb_process_time* pt, const int32_
   return upload_voice_map(pt->G, voice_instrument, n_voices, pt->d_vmap, &pt->V);
 }
 
+static int beat_phase_plane_check(int plane0, int n_planes)
+{
+  return plane0 < 0 || n_planes <= plane0
+             ? fail(MLB_ERR_INVALID, "beat-phase plane %d is not within the %d output planes", plane0, n_planes)
+             : MLB_OK;
+}
+
 extern "C" int mlb_process_time_process_device(mlb_process_time* pt, const int32_t* offsets_dev,
                                                const mlb_transport* transports_dev, float* out_dev, int plane0,
                                                int n_planes, int n_blocks, void* stream)
 {
   if (!pt || !offsets_dev || !out_dev) return fail(MLB_ERR_INVALID, "null argument");
   if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive (got %d)", n_blocks);
-  if (plane0 < 0 || n_planes <= plane0)
-    return fail(MLB_ERR_INVALID, "beat-phase plane %d is not within the %d output planes", plane0, n_planes);
+  MLB_TRY(beat_phase_plane_check(plane0, n_planes));
   PtArgs a;
-  a.offsets = offsets_dev, a.tr = transports_dev, a.state = pt->d_state.get(), a.out = out_dev;
-  a.vmap_off = pt->V ? pt->d_vmap.get() : nullptr;
-  a.vmap_voice = pt->V ? pt->d_vmap.get() + pt->G + 2 : nullptr;
-  a.G = pt->G, a.N = pt->V ? pt->V : pt->G, a.T = n_blocks;
-  a.plane0 = plane0, a.n_planes = n_planes;
-  a.n_gblk = (pt->G + 31) / 32;
+  list_bank_args(*pt, a, offsets_dev, out_dev, plane0, n_planes, n_blocks);
+  a.tr = transports_dev, a.state = pt->d_state.get();
   process_time_kernel<<<(unsigned)((a.n_gblk + kPtWarps - 1) / kPtWarps), 32 * kPtWarps, 0, (cudaStream_t)stream>>>(a);
   ++g_launches;
   CU_CHECK(cudaGetLastError());
@@ -3047,28 +3079,9 @@ extern "C" int mlb_process_time_process_host(mlb_process_time* pt, const int32_t
   if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive (got %d)", n_blocks);
   if (n_transports < 0) return fail(MLB_ERR_INVALID, "n_transports must not be negative (got %d)", n_transports);
   MLB_TRY(check_offsets(offsets_host, pt->G, n_transports, n_blocks, "transport", "updates"));
-  if (plane0 < 0 || n_planes <= plane0)
-    return fail(MLB_ERR_INVALID, "beat-phase plane %d is not within the %d output planes", plane0, n_planes);
-  const size_t T = (size_t)n_blocks, N = pt->V ? pt->V : pt->G;
-  const size_t off_bytes = T * (pt->G + 1) * 4, tr_bytes = (size_t)n_transports * sizeof(mlb_transport);
-  MLB_TRY(pt->d_off.ensure(off_bytes, "staging"));
-  if (n_transports) MLB_TRY(pt->d_tr.ensure(tr_bytes, "staging"));
-  MLB_TRY(pt->d_out.ensure(T * n_planes * N * MLB_BLOCK * 4, "staging"));
-  cudaStream_t s = pt->stream.get();
-  const int rc = [&]() -> int
-  {
-    CU_CHECK(cudaMemcpyAsync(pt->d_off.get(), offsets_host, off_bytes, cudaMemcpyHostToDevice, s));
-    if (n_transports) CU_CHECK(cudaMemcpyAsync(pt->d_tr.get(), transports_host, tr_bytes, cudaMemcpyHostToDevice, s));
-    MLB_TRY(mlb_process_time_process_device(pt, pt->d_off.get(), pt->d_tr.get(), pt->d_out.get(), plane0, n_planes,
-                                            n_blocks, s));
-    // only the phase plane comes down: the caller's other planes stay as they were
-    const size_t plane = N * MLB_BLOCK * 4, pitch = (size_t)n_planes * plane;
-    CU_CHECK(cudaMemcpy2DAsync(reinterpret_cast<char*>(out_host) + plane0 * plane, pitch,
-                               reinterpret_cast<const char*>(pt->d_out.get()) + plane0 * plane, pitch, plane, T,
-                               cudaMemcpyDeviceToHost, s));
-    return MLB_OK;
-  }();
-  return drain(rc, {s});
+  MLB_TRY(beat_phase_plane_check(plane0, n_planes));
+  return list_bank_host(pt, mlb_process_time_process_device, pt->d_tr, offsets_host, transports_host, n_transports,
+                        out_host, plane0, 1, n_planes, n_blocks);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -3259,8 +3272,7 @@ extern "C" int mlb_routers_process_host(mlb_routers* r, const int32_t* offsets_h
   cudaStream_t s = r->stream.get();
   const int rc = [&]() -> int
   {
-    CU_CHECK(cudaMemcpyAsync(r->d_off.get(), offsets_host, T * G1 * 4, cudaMemcpyHostToDevice, s));
-    if (n_events) CU_CHECK(cudaMemcpyAsync(r->d_ev.get(), events_host, n_events * sizeof(mlb_event), cudaMemcpyHostToDevice, s));
+    CU_CHECK(upload_list_chunk(r->d_off.get(), offsets_host, G1, r->d_ev.get(), events_host, n_events, 0, n_blocks, s));
     MLB_TRY(mlb_routers_process_device(r, r->d_off.get(), r->d_ev.get(), r->d_rec.get(), r->d_coff.get(), r->d_ch.get(),
                                        n_blocks, s));
     CU_CHECK(cudaMemcpyAsync(records_host, r->d_rec.get(), T * r->V * sizeof(mlb_voice_events), cudaMemcpyDeviceToHost, s));
@@ -3316,19 +3328,6 @@ static int synth_routed(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb, mlb
   c.r = r, c.offsets = offsets_host, c.events = events_host, c.n_events = n_events, c.n_changes = n_changes, c.cb = cb;
   c.pt = pt, c.time_offsets = time_offsets_host, c.transports = transports_host, c.n_transports = n_transports;
   return c.run();
-}
-
-// Rows [t0, t1) of a [T][G + 1] offset table into the same rows of dev_off, and with the first chunk the whole list of
-// n items it indexes into dev_items.
-template <class Item>
-static cudaError_t upload_list_chunk(int32_t* dev_off, const int32_t* off, size_t G1, Item* dev_items, const Item* items,
-                                     int n, int t0, int t1, cudaStream_t s)
-{
-  cudaError_t e = cudaSuccess;
-  if (t0 == 0 && n) e = cudaMemcpyAsync(dev_items, items, n * sizeof(Item), cudaMemcpyHostToDevice, s);
-  if (e == cudaSuccess)
-    e = cudaMemcpyAsync(dev_off + t0 * G1, off + t0 * G1, (t1 - t0) * G1 * 4, cudaMemcpyHostToDevice, s);
-  return e;
 }
 
 // The contract-E driver, on host_pipeline over time chunks of Tc blocks: the chunk's records or raw-event offsets, and
