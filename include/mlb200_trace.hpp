@@ -46,6 +46,7 @@
 #include <cstring>
 #include <functional>
 #include <map>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -86,6 +87,12 @@ class Recorder
   int forbidFunctors = 0;       // > 0 inside a Downsample2xFunction's process function (see there)
   int pendingAgain = -1;        // node of the functor's first call in this pass
   int* pendingOwner = nullptr;  // where a functor's first call wants its node index written
+  // TracedSynth::trace: the voice being traced, and the voice each functor object was first called by
+  int voice = -1;
+  std::map<const void*, int>* functorVoice = nullptr;
+  // TracedSynth::trace: the one pass whose symbols may be read stale (pass 1 of this voice, while pass 2 runs); -2:
+  // none.  -1 (TracedProcessor): any earlier pass.
+  int staleEpoch = -1;
 
   static Recorder*& current()
   {
@@ -183,6 +190,22 @@ class DSPVector
     }
     if (epoch == r.epoch) return node;
     // a symbol of the previous pass: state the caller keeps between process calls
+    if (r.staleEpoch != -1)
+    {
+      // a voice's own member is written only in its own two passes; anything older was written by another voice
+      if (epoch != r.staleEpoch)
+        throw Error(MLB_ERR_UNSUPPORTED,
+                    ("mlb::tr::TracedSynth: voice " + std::to_string(r.voice) +
+                     " reads a DSPVector of another voice (a member shared between voices, or another voice's Voice "
+                     "rows); a row carried between vectors must be per voice, e.g. DSPVector carried[16]")
+                        .c_str());
+      if (opIndex < 0)
+        throw Error(MLB_ERR_UNSUPPORTED,
+                    ("mlb::tr::TracedSynth: voice " + std::to_string(r.voice) +
+                     " carries a Voice row, controller, beat phase or tr::param between vectors as it stands; carry "
+                     "an expression of it (e.g. row * 1.f)")
+                        .c_str());
+    }
     auto it = r.feedbackReaders.find(opIndex);
     if (it != r.feedbackReaders.end()) return it->second;
     const int n = r.addNode(MLB_OP_FEEDBACK_READ, {}, 0, false);
@@ -517,6 +540,15 @@ class Functor
       throw Error(MLB_ERR_UNSUPPORTED,
                   "mlb::tr: the process function of a Downsample2xFunction must be stateless (its functors would have to "
                   "tick on every second vector only)");
+    if (r.functorVoice)
+    {
+      // in the reference one object shared by two voices ticks once per voice and vector; each lane here has its own
+      auto it = r.functorVoice->emplace(this, r.voice).first;
+      if (it->second != r.voice)
+        throw Error(MLB_ERR_UNSUPPORTED, ("mlb::tr: a functor object is called by voice " + std::to_string(it->second) +
+                                          " and voice " + std::to_string(r.voice) + "; each voice needs its own")
+                                             .c_str());
+    }
     if (lastEpoch_ == r.epoch)
     {
       // called again in the same vector: the reference object would simply tick once more (a process function run twice
@@ -1368,6 +1400,47 @@ class DSPVectorDynamic
 using MainInputs = const DSPVectorDynamic&;
 using MainOutputs = DSPVectorDynamic&;
 
+// ---- the synth spelling: EventsToSignals' voice rows (MLEventsToSignals.h:15-26, 46-47, 184) ----
+enum VoiceOutputSignals
+{
+  kPitch = 0,
+  kGate,
+  kVoice,
+  kZ,
+  kX,
+  kY,
+  kMod,
+  kElapsedTime,
+  kNumVoiceOutputRows
+};
+
+class EventsToSignals
+{
+ public:
+  static constexpr size_t kMaxVoices{16};
+  struct Voice
+  {
+    DSPVectorArray<kNumVoiceOutputRows> outputs;  // symbolic: INPUT planes 0..7 of the traced graph
+  };
+};
+
+using Symbol = std::string;  // what setInputProtocol takes ("MIDI" or "MPE")
+
+// MLSynth.h:16-19, a host scalar
+inline float pitchToFrequency(float pitch) { return 440.0f * powf(2.0f, (pitch - 69.0f) / 12.0f); }
+
+// what getInputVoice / getInputController / getBeatPhase return while TracedSynth::trace runs one voice
+struct SynthPass
+{
+  static constexpr int kPhasePlane = 1 << 20;  // INPUT iarg of the beat phase until the controller count is known
+  static constexpr int kAccPlane = 1 << 21;    // INPUT iarg kAccPlane + i: the accumulator outputs[i] at entry
+  int voice = -1;
+  EventsToSignals::Voice rows;
+  std::vector<int>* controllers = nullptr;  // controller numbers in first-use order, over all voices
+  std::map<int, int> controllerNode;        // this pass: controller number -> its INPUT node
+  int phaseNode = -1;
+};
+
 class AudioContext
 {
   double sampleRate_ = 0;
@@ -1378,8 +1451,121 @@ class AudioContext
   void setSampleRate(int r) { sampleRate_ = r; }
   DSPVectorDynamic inputs;
   DSPVectorDynamic outputs;
+
+  // The instrument settings a synth's setup makes (MLAudioContext.h:76-98): recorded here, applied to every instrument
+  // by TracedSynth::compile.  The defaults are EventsToSignals' (MLEventsToSignals.h:213-228).
+  struct InputSettings
+  {
+    int polyphony = 0;
+    bool mpe = false;
+    bool unison = false;
+    int modCC = 16;
+    float pitchBend = 7.f, mpePitchBend = 24.f, glideSeconds = 0.f, driftAmount = 0.f;
+  };
+  InputSettings input;
+  void setInputPolyphony(int voices) { input.polyphony = voices; }
+  void setInputProtocol(const Symbol& p)
+  {
+    if (p != "MIDI" && p != "MPE") throw Error(MLB_ERR_INVALID, ("mlb::tr: protocol " + p + " is not MIDI or MPE").c_str());
+    input.mpe = p == "MPE";
+  }
+  void setInputUnison(bool u) { input.unison = u; }
+  void setInputModCC(int p) { input.modCC = p; }
+  void setInputPitchBend(float p) { input.pitchBend = p; }
+  void setInputMPEPitchBend(float p) { input.mpePitchBend = p; }
+  void setInputGlideTimeInSeconds(float s) { input.glideSeconds = s; }
+  void setInputDriftAmount(float d) { input.driftAmount = d; }
+
+  // the voice's rows, a smoothed controller, the beat phase: symbolic rows (INPUT planes 0..7, 8 + k, 8 + C)
+  const EventsToSignals::Voice& getInputVoice(int n)
+  {
+    if (!pass_) throw Error(MLB_ERR_INVALID, "mlb::tr: getInputVoice outside TracedSynth::trace()");
+    if (n != pass_->voice)
+      throw Error(MLB_ERR_UNSUPPORTED, ("mlb::tr: voice " + std::to_string(pass_->voice) + " reads the rows of voice " +
+                                        std::to_string(n) + "; a voice may read only its own rows")
+                                           .c_str());
+    return pass_->rows;
+  }
+  DSPVector getInputController(size_t n) const
+  {
+    if (!pass_) throw Error(MLB_ERR_INVALID, "mlb::tr: getInputController outside TracedSynth::trace()");
+    if (n > 128)
+      throw Error(MLB_ERR_INVALID, ("mlb::tr: controller " + std::to_string(n) + " is above 128 (EventsToSignals has 129)").c_str());
+    auto it = pass_->controllerNode.find((int)n);
+    if (it == pass_->controllerNode.end())
+    {
+      std::vector<int>& list = *pass_->controllers;
+      size_t k = 0;
+      while (k < list.size() && list[k] != (int)n) ++k;
+      if (k == list.size()) list.push_back((int)n);
+      Recorder& r = Recorder::get();
+      it = pass_->controllerNode.emplace((int)n, r.addNode(MLB_OP_INPUT, {}, MLB_VOICE_ROWS + (int)k, false)).first;
+    }
+    return DSPVector::ofNode(it->second);
+  }
+  DSPVector getBeatPhase()
+  {
+    if (!pass_) throw Error(MLB_ERR_INVALID, "mlb::tr: getBeatPhase outside TracedSynth::trace()");
+    if (pass_->phaseNode < 0) pass_->phaseNode = Recorder::get().addNode(MLB_OP_INPUT, {}, SynthPass::kPhasePlane, false);
+    return DSPVector::ofNode(pass_->phaseNode);
+  }
+
+  SynthPass* pass_ = nullptr;  // set by TracedSynth::trace
 };
 using SignalProcessFn = void (*)(AudioContext*, void*);
+
+// MLSignalProcessor.h: the base of Synth, reduced to what a Synth subclass uses
+class SignalProcessor
+{
+ public:
+  SignalProcessor() {}
+  virtual ~SignalProcessor() {}
+  virtual void processVector(const DSPVectorDynamic& inputs, DSPVectorDynamic& outputs, void* stateData = nullptr) {}
+  virtual void setSampleRate(double sr) { sampleRate_ = sr; }
+
+ protected:
+  double sampleRate_{0};
+};
+
+// Synth (MLSynth.h:26-93): subclasses implement processVoice; TracedSynth traces it once per voice
+class Synth : public SignalProcessor
+{
+ public:
+  static constexpr int kDefaultNumVoices = 8;
+  static constexpr int kNumVoices = 8;
+
+  Synth(int numVoices = kDefaultNumVoices) : numVoices_(numVoices) {}
+  virtual ~Synth() = default;
+
+  void processVector(const DSPVectorDynamic& inputs, DSPVectorDynamic& outputs, void* stateData) override
+  {
+    auto* audioContext = static_cast<AudioContext*>(stateData);
+    if (!audioContext) return;
+    for (int i = 0; i < (int)outputs.size(); ++i) outputs[i] = DSPVector{0.f};
+    int activeCount = 0;
+    for (int v = 0; v < numVoices_; ++v)
+    {
+      const auto& voice = audioContext->getInputVoice(v);
+      if (isVoiceActive(v, voice))
+      {
+        activeCount++;
+        processVoice(v, voice, inputs, outputs, audioContext);
+      }
+    }
+    activeVoiceCount_ = activeCount;
+  }
+
+  virtual void processVoice(int voiceIndex, const EventsToSignals::Voice& voice, const DSPVectorDynamic& inputs,
+                            DSPVectorDynamic& outputs, AudioContext* audioContext) = 0;
+  virtual bool isVoiceActive(int voiceIndex, const EventsToSignals::Voice& voice) { return true; }
+  int getActiveVoiceCount() const { return activeVoiceCount_; }
+  int getNumVoices() const { return numVoices_; }
+  virtual bool hasActiveVoices() const { return activeVoiceCount_ > 0; }
+
+ protected:
+  int numVoices_;
+  int activeVoiceCount_ = 0;
+};
 
 // ------------------------------------------------------------------------------------------------------
 // TracedProcessor: trace a SignalProcessFn, compile it for `instances` independent copies, run it on the GPU.
@@ -1567,6 +1753,443 @@ class TracedProcessor
 
  private:
   std::vector<float> bcast_;
+};
+
+// ------------------------------------------------------------------------------------------------------
+// TracedSynth: trace a Synth subclass's processVoice, compile it for G instruments, run it from raw events.
+//
+// processVoice is traced once per voice (two passes each, as TracedProcessor::trace, so carried DSPVector members
+// become feedback edges).  At entry every outputs[i] is an accumulator; a voice must leave it untouched or end it as
+// the accumulator plus ONE expression x.  Graph output i is x (or a +0 row), and the bus kernel sums the voices of an
+// instrument as ((+0 + x0) + x1) + ..., which is what Synth::processVector's `outputs[i] = 0; outputs[i] += ...` gives
+// in voice order.  All voices must record the same nodes; their coefficient and state words may differ (a cutoff
+// that depends on voiceIndex) and become per-lane words.  The graph's INPUT planes follow contract E: the Voice rows
+// at 0..7, the controllers a voice reads at 8 + k in first-use order, the beat phase after them.
+class TracedSynth
+{
+  struct VoiceGraph
+  {
+    std::vector<TNode> nodes;
+    std::vector<int32_t> outs;
+  };
+  std::vector<VoiceGraph> voices_;  // one per synth voice
+  std::vector<mlb_node> nodes_;
+  std::vector<int32_t> outs_, stOff_, coOff_;
+  mlb_layout layout_{};
+  std::vector<int> controllers_;
+  bool phase_ = false;
+  AudioContext::InputSettings settings_;
+  double sampleRate_ = 0;
+  int numVoices_ = 0;
+  size_t nOut_ = 0;
+
+  int instruments_ = 0, lanesPer_ = 0;
+  std::vector<float> coef_;
+  std::vector<uint32_t> state_;
+  mlb_graph* g_ = nullptr;
+  std::unique_ptr<RouterBank> routers_;
+  std::unique_ptr<VoiceBank> voiceBank_;
+  std::unique_ptr<ControllerBank> ctrl_;
+  std::unique_ptr<ProcessTimeBank> times_;
+  std::unique_ptr<Buses> buses_;
+  std::vector<int64_t> overflow_;  // the router bank's overflow counts after the last call
+
+  [[noreturn]] static void refuse(int v, const std::string& what)
+  {
+    throw Error(MLB_ERR_UNSUPPORTED, ("mlb::tr::TracedSynth: voice " + std::to_string(v) + " " + what).c_str());
+  }
+
+  // the pass's graph without the accumulators and unread Voice rows; out i = x, or -1 for an untouched output
+  static VoiceGraph extract(const Recorder& rec, const std::vector<int>& acc, const std::vector<int>& fin, int v)
+  {
+    const int n = (int)rec.nodes.size(), nOut = (int)acc.size();
+    std::vector<char> drop((size_t)n, 0);
+    std::vector<int> accOf((size_t)n, -1), x((size_t)nOut, -1);
+    for (int i = 0; i < nOut; ++i) drop[(size_t)acc[(size_t)i]] = 1, accOf[(size_t)acc[(size_t)i]] = i;
+    const auto name = [](int i) { return "outputs[" + std::to_string(i) + "]"; };
+    for (int i = 0; i < nOut; ++i)
+    {
+      const int f = fin[(size_t)i];
+      if (f == acc[(size_t)i]) continue;  // untouched
+      const mlb_node& m = rec.nodes[(size_t)f].node;
+      if (m.op == MLB_OP_ADD && m.in[0] == acc[(size_t)i] && !drop[(size_t)f])
+      {
+        drop[(size_t)f] = 1, x[(size_t)i] = m.in[1];
+        continue;
+      }
+      if (m.op == MLB_OP_ADD && m.in[0] >= 0 && rec.nodes[(size_t)m.in[0]].node.op == MLB_OP_ADD &&
+          rec.nodes[(size_t)m.in[0]].node.in[0] == acc[(size_t)i])
+        refuse(v, "adds twice into " + name(i) + ": (acc + a) + b is not one bus term; add one expression");
+      if (accOf[(size_t)f] >= 0) refuse(v, "assigns " + name(accOf[(size_t)f]) + " to " + name(i));
+      bool reads = false;
+      for (const TNode& t : rec.nodes)
+        for (int k = 0; k < MLB_MAX_INS; ++k) reads = reads || t.node.in[k] == acc[(size_t)i];
+      if (reads)
+        refuse(v, "reads or rescales the accumulator " + name(i) + "; only " + name(i) + " += x (accumulator + x) is "
+                  "allowed: x + " + name(i) + " keeps x's NaN payload where the reference keeps the accumulator's");
+      refuse(v, "assigns " + name(i) + " = x; a voice adds into its outputs: " + name(i) + " += x");
+    }
+    std::vector<int> uses((size_t)n, 0);
+    for (int j = 0; j < n; ++j)
+    {
+      if (drop[(size_t)j]) continue;
+      const mlb_node& m = rec.nodes[(size_t)j].node;
+      for (int k = 0; k < MLB_MAX_INS; ++k)
+      {
+        const int s = m.in[k];
+        if (s < 0) continue;
+        if (accOf[(size_t)s] >= 0) refuse(v, "reads or rescales the accumulator " + name(accOf[(size_t)s]));
+        if (drop[(size_t)s]) refuse(v, "reads an output after adding into it");
+        ++uses[(size_t)s];
+      }
+    }
+    for (int i = 0; i < nOut; ++i)
+    {
+      const int s = x[(size_t)i];
+      if (s < 0) continue;
+      if (accOf[(size_t)s] >= 0) refuse(v, "adds the accumulator " + name(accOf[(size_t)s]) + " into " + name(i));
+      if (drop[(size_t)s]) refuse(v, "adds one output into another");
+      ++uses[(size_t)s];
+    }
+    for (int j = 0; j < n; ++j)  // Voice rows the voice does not read
+    {
+      const mlb_node& m = rec.nodes[(size_t)j].node;
+      if (m.op == MLB_OP_INPUT && m.iarg < MLB_VOICE_ROWS && uses[(size_t)j] == 0) drop[(size_t)j] = 1;
+    }
+    std::vector<int> idx((size_t)n, -1);
+    VoiceGraph vg;
+    for (int j = 0; j < n; ++j)
+      if (!drop[(size_t)j]) idx[(size_t)j] = (int)vg.nodes.size(), vg.nodes.push_back(rec.nodes[(size_t)j]);
+    for (TNode& t : vg.nodes)
+    {
+      for (int k = 0; k < MLB_MAX_INS; ++k)
+        if (t.node.in[k] >= 0) t.node.in[k] = idx[(size_t)t.node.in[k]];
+      if (t.node.op == MLB_OP_FEEDBACK_WRITE) t.node.iarg = idx[(size_t)t.node.iarg];
+      else if (TracedProcessor::isAgain(t.node)) t.node.iarg = MLB_AGAIN(idx[(size_t)MLB_AGAIN_TARGET(t.node.iarg)]);
+    }
+    for (int i = 0; i < nOut; ++i) vg.outs.push_back(x[(size_t)i] < 0 ? -1 : idx[(size_t)x[(size_t)i]]);
+    return vg;
+  }
+
+  static bool sameStructure(const VoiceGraph& a, const VoiceGraph& b, std::string& where)
+  {
+    if (a.nodes.size() != b.nodes.size()) return where = "a different number of nodes", false;
+    if (a.outs != b.outs) return where = "different outputs", false;
+    for (size_t j = 0; j < a.nodes.size(); ++j)
+    {
+      const mlb_node &p = a.nodes[j].node, &q = b.nodes[j].node;
+      bool same = p.op == q.op && p.iarg == q.iarg && a.nodes[j].name == b.nodes[j].name;
+      for (int k = 0; k < MLB_MAX_INS; ++k) same = same && p.in[k] == q.in[k];
+      if (!same) return where = "node " + std::to_string(j), false;
+    }
+    return true;
+  }
+
+  // synth voice of lane j of an instrument (MPE lane 0 is the main voice, which no voice reads: voice 0's words)
+  int laneVoice(int j) const
+  {
+    const int v = settings_.mpe ? j - 1 : j;
+    return v >= 0 && v < numVoices_ ? v : 0;
+  }
+  int lane(int instrument, int voice) const { return instrument * lanesPer_ + (settings_.mpe ? 1 : 0) + voice; }
+
+ public:
+  TracedSynth() = default;
+  ~TracedSynth()
+  {
+    if (g_) mlb_graph_destroy(g_);
+  }
+  TracedSynth(const TracedSynth&) = delete;
+  TracedSynth& operator=(const TracedSynth&) = delete;
+
+  // Record processVoice for every voice of `synth` (host only: works without a GPU).  `ctx` carries the instrument
+  // settings the synth's setup made (setInputPolyphony, ...) and the sample rate; its outputs are the synth's outputs.
+  void trace(Synth& synth, AudioContext& ctx)
+  {
+    const int V = synth.getNumVoices();
+    const int P = ctx.input.polyphony;
+    if (ctx.inputs.size() != 0)
+      throw Error(MLB_ERR_UNSUPPORTED, "mlb::tr::TracedSynth: the synth has audio inputs; only synths without inputs are traced");
+    if (V < 1) throw Error(MLB_ERR_INVALID, "mlb::tr::TracedSynth: the synth has no voices");
+    if (P < V || P > (int)EventsToSignals::kMaxVoices)
+      throw Error(MLB_ERR_UNSUPPORTED,
+                  ("mlb::tr::TracedSynth: polyphony " + std::to_string(P) + " must be in [getNumVoices() = " +
+                   std::to_string(V) + ", 16]: EventsToSignals runs only voices 1..polyphony; call setInputPolyphony(" +
+                   std::to_string(V) + ")")
+                      .c_str());
+    if (ctx.input.driftAmount != 0.f)
+      throw Error(MLB_ERR_UNSUPPORTED,
+                  ("mlb::tr::TracedSynth: drift amount " + std::to_string(ctx.input.driftAmount) +
+                   " is not 0: EventsToSignals starts an instrument's voices, drift included, only at its first event "
+                   "(awake_), and the device Voice bank runs them from the first vector; call setInputDriftAmount(0)")
+                      .c_str());
+    if (ctx.input.modCC < 0 || ctx.input.modCC > 127)
+      throw Error(MLB_ERR_INVALID, ("mlb::tr::TracedSynth: mod CC " + std::to_string(ctx.input.modCC) + " is not in 0..127").c_str());
+    Recorder rec;
+    std::map<const void*, int> functorVoice;
+    std::vector<int> controllers;
+    bool phase = false;
+    std::vector<VoiceGraph> graphs;
+    std::vector<SynthPass> passes((size_t)V);  // kept for the whole trace: a Voice& held by a later voice stays valid
+    Recorder*& cur = Recorder::current();
+    Recorder* prev = cur;
+    cur = &rec;
+    rec.functorVoice = &functorVoice;
+    try
+    {
+      for (int v = 0; v < V; ++v)
+      {
+        SynthPass& pass = passes[(size_t)v];
+        std::vector<int> acc, fin;
+        rec.voice = v;
+        for (int p = 0; p < 2; ++p)  // pass 1 finds which symbols survive the call; pass 2 is the graph
+        {
+          rec.staleEpoch = p == 0 ? -2 : rec.epoch;  // pass 2 may read what pass 1 of this voice left
+          rec.beginPass();
+          pass.voice = v;
+          pass.controllers = &controllers;
+          pass.controllerNode.clear();
+          pass.phaseNode = -1;
+          for (int r = 0; r < kNumVoiceOutputRows; ++r)
+            pass.rows.outputs.row(r) = DSPVector::ofNode(rec.addNode(MLB_OP_INPUT, {}, r, false));
+          acc.clear();
+          for (size_t i = 0; i < ctx.outputs.size(); ++i)
+          {
+            acc.push_back(rec.addNode(MLB_OP_INPUT, {}, SynthPass::kAccPlane + (int)i, false));
+            ctx.outputs[i] = DSPVector::ofNode(acc.back());
+          }
+          ctx.pass_ = &pass;
+          if (!synth.isVoiceActive(v, ctx.getInputVoice(v)))
+            refuse(v, "is not active (isVoiceActive returned false); every voice is processed on every vector");
+          synth.processVoice(v, ctx.getInputVoice(v), ctx.inputs, ctx.outputs, &ctx);
+          ctx.pass_ = nullptr;
+        }
+        for (const auto& fr : rec.feedbackReaders)
+        {
+          auto it = rec.opIndexToNode.find(fr.first);
+          if (it == rec.opIndexToNode.end()) throw Error(MLB_ERR_INVALID, "mlb::tr: processVoice is not deterministic between calls");
+          rec.addNode(MLB_OP_FEEDBACK_WRITE, {it->second}, fr.second, false);
+        }
+        fin.clear();
+        for (size_t i = 0; i < ctx.outputs.size(); ++i) fin.push_back(ctx.outputs[i].resolve());
+        phase = phase || pass.phaseNode >= 0;
+        graphs.push_back(extract(rec, acc, fin, v));
+        std::string where;
+        if (v > 0 && !sameStructure(graphs[0], graphs.back(), where))
+          refuse(v, "records a different graph from voice 0 (" + where +
+                        "); voices may differ in coefficients and state only");
+      }
+    }
+    catch (...)
+    {
+      ctx.pass_ = nullptr;
+      rec.active = false;
+      cur = prev;
+      throw;
+    }
+    rec.active = false;
+    cur = prev;
+    // the beat phase after the controllers; untouched outputs read one shared +0 row
+    const int phasePlane = MLB_VOICE_ROWS + (int)controllers.size();
+    for (VoiceGraph& vg : graphs)
+    {
+      for (TNode& t : vg.nodes)
+        if (t.node.op == MLB_OP_INPUT && t.node.iarg == SynthPass::kPhasePlane) t.node.iarg = phasePlane;
+      int zero = -1;
+      for (int32_t& o : vg.outs)
+        if (o < 0)
+        {
+          if (zero < 0)
+          {
+            TNode z;
+            z.node.op = MLB_OP_PARAM;
+            for (int k = 0; k < MLB_MAX_INS; ++k) z.node.in[k] = -1;
+            z.node.iarg = 0;
+            z.coef.assign(1, 0.f);
+            zero = (int)vg.nodes.size();
+            vg.nodes.push_back(z);
+          }
+          o = zero;
+        }
+    }
+    voices_ = std::move(graphs);
+    controllers_ = controllers;
+    phase_ = phase;
+    settings_ = ctx.input;
+    sampleRate_ = ctx.getSampleRate();
+    numVoices_ = V;
+    nOut_ = ctx.outputs.size();
+    nodes_.clear();
+    for (const TNode& t : voices_[0].nodes) nodes_.push_back(t.node);
+    outs_ = voices_[0].outs;
+    stOff_.assign(nodes_.size(), 0);
+    coOff_.assign(nodes_.size(), 0);
+    check(mlb_graph_layout(nodes_.data(), (int)nodes_.size(), &layout_, stOff_.data(), coOff_.data()));
+  }
+
+  const std::vector<mlb_node>& nodes() const { return nodes_; }
+  const std::vector<int32_t>& outs() const { return outs_; }
+  const std::vector<int>& controllers() const { return controllers_; }
+  bool readsBeatPhase() const { return phase_; }
+  const AudioContext::InputSettings& settings() const { return settings_; }
+  int numVoices() const { return numVoices_; }
+  // lanes of one instrument: polyphony voices, plus the MPE main voice first
+  int lanesPerInstrument() const { return settings_.polyphony + (settings_.mpe ? 1 : 0); }
+
+  // JSON: nodes (with every voice's coefficient and state words), outs, controllers, beat phase, settings -- what a
+  // test or a tool needs to rebuild the instrument bank elsewhere (tests/test_synth_trace.py).
+  void dump(FILE* f) const
+  {
+    const AudioContext::InputSettings& s = settings_;
+    std::fprintf(f, "{\"n_voices\": %d, \"sample_rate\": %.17g, \"polyphony\": %d, \"mpe\": %d, \"unison\": %d, "
+                    "\"mod_cc\": %d, \"pitch_bend\": %.9g, \"mpe_pitch_bend\": %.9g, \"glide_seconds\": %.9g, "
+                    "\"drift_amount\": %.9g, \"phase\": %d, \"controllers\": [",
+                 numVoices_, sampleRate_, s.polyphony, (int)s.mpe, (int)s.unison, s.modCC, s.pitchBend, s.mpePitchBend,
+                 s.glideSeconds, s.driftAmount, (int)phase_);
+    for (size_t k = 0; k < controllers_.size(); ++k) std::fprintf(f, "%s%d", k ? ", " : "", controllers_[k]);
+    std::fprintf(f, "], \"nodes\": [");
+    for (size_t i = 0; i < nodes_.size(); ++i)
+    {
+      const mlb_node& m = nodes_[i];
+      std::fprintf(f, "%s{\"op\": %d, \"in\": [", i ? ", " : "", m.op);
+      for (int k = 0; k < MLB_MAX_INS; ++k) std::fprintf(f, "%s%d", k ? ", " : "", m.in[k]);
+      std::fprintf(f, "], \"iarg\": %d, \"name\": \"%s\", \"coef\": [", m.iarg, voices_[0].nodes[i].name.c_str());
+      const bool again = TracedProcessor::isAgain(m);  // a further call of an earlier functor owns no words
+      for (size_t v = 0; v < voices_.size(); ++v)
+      {
+        const TNode& t = voices_[v].nodes[i];
+        std::fprintf(f, "%s[", v ? ", " : "");
+        for (size_t k = 0; k < t.coef.size() && !again; ++k)
+        {
+          uint32_t u;
+          std::memcpy(&u, &t.coef[k], 4);
+          std::fprintf(f, "%s%u", k ? ", " : "", u);
+        }
+        std::fprintf(f, "]");
+      }
+      std::fprintf(f, "], \"state\": [");
+      for (size_t v = 0; v < voices_.size(); ++v)
+      {
+        const TNode& t = voices_[v].nodes[i];
+        std::fprintf(f, "%s[", v ? ", " : "");
+        for (size_t k = 0; k < t.state.size() && !again; ++k) std::fprintf(f, "%s%u", k ? ", " : "", t.state[k]);
+        std::fprintf(f, "]");
+      }
+      std::fprintf(f, "]}");
+    }
+    std::fprintf(f, "], \"outs\": [");
+    for (size_t i = 0; i < outs_.size(); ++i) std::fprintf(f, "%s%d", i ? ", " : "", outs_[i]);
+    std::fprintf(f, "]}\n");
+  }
+
+  // Create the banks for `instruments` instruments (needs a GPU): the router and Voice bank over
+  // instruments x lanesPerInstrument() lanes, the controller and beat-phase banks if processVoice reads them, the
+  // graph over every lane, and one bus per instrument over its getNumVoices() voices (never the MPE main voice).
+  void compile(int instruments, unsigned flags = MLB_GRAPH_EXACT)
+  {
+    if (nodes_.empty()) throw Error(MLB_ERR_INVALID, "mlb::tr::TracedSynth: trace() first");
+    if (instruments < 1) throw Error(MLB_ERR_INVALID, "mlb::tr::TracedSynth: instruments must be positive");
+    if (g_) mlb_graph_destroy(g_), g_ = nullptr;
+    buses_.reset(), times_.reset(), ctrl_.reset(), voiceBank_.reset(), routers_.reset();
+    const AudioContext::InputSettings& s = settings_;
+    const int G = instruments, NR = lanesPerInstrument(), V = G * NR;
+    instruments_ = G, lanesPer_ = NR;
+    std::vector<int32_t> poly((size_t)G, s.polyphony), first((size_t)G), unison((size_t)G, s.unison ? 1 : 0),
+        modCC((size_t)G, s.modCC), busFirst((size_t)G), busCount((size_t)G, numVoices_);
+    std::vector<int32_t> vi((size_t)V), mainVoice((size_t)V, -1), inst((size_t)V);
+    std::vector<float> glide((size_t)V, s.glideSeconds), drift((size_t)V, s.driftAmount), bend((size_t)V, s.pitchBend);
+    for (int g = 0; g < G; ++g)
+    {
+      first[(size_t)g] = g * NR, busFirst[(size_t)g] = lane(g, 0);
+      for (int j = 0; j < NR; ++j)
+      {
+        const size_t l = (size_t)(g * NR + j);
+        vi[l] = s.mpe ? j : j + 1;
+        inst[l] = g;
+        if (s.mpe && j > 0) mainVoice[l] = g * NR, bend[l] = s.mpePitchBend;
+      }
+    }
+    const float sr = (float)sampleRate_;
+    routers_.reset(new RouterBank(G, s.mpe ? 1 : 0, poly.data(), first.data(), V, unison.data(), modCC.data()));
+    voiceBank_.reset(new VoiceBank(V, sr, vi.data(), glide.data(), drift.data(), bend.data(), s.mpe ? 0u : MLB_VOICES_MIDI));
+    if (s.mpe) voiceBank_->setMainVoices(mainVoice.data());
+    if (!controllers_.empty())
+    {
+      ctrl_.reset(new ControllerBank(G, sr, s.mpe ? 1 : 0, controllers_.data(), (int)controllers_.size()));
+      ctrl_->setVoiceMap(inst.data(), V);
+    }
+    if (phase_)
+    {
+      times_.reset(new ProcessTimeBank(G, sampleRate_));
+      times_->setVoiceMap(inst.data(), V);
+    }
+    check(mlb_graph_create(nodes_.data(), (int)nodes_.size(), outs_.data(), (int)outs_.size(), V, flags, &g_));
+    buses_.reset(new Buses(V, G, busFirst.data(), busCount.data()));
+    overflow_.assign((size_t)G, 0);
+    coef_.assign((size_t)layout_.n_coef_words * V, 0.f);
+    state_.assign((size_t)layout_.n_state_words * V, 0u);
+    for (size_t i = 0; i < nodes_.size(); ++i)
+    {
+      if (TracedProcessor::isAgain(nodes_[i])) continue;  // the words belong to the functor's first call
+      for (int l = 0; l < V; ++l)
+      {
+        const TNode& t = voices_[(size_t)laneVoice(l % NR)].nodes[i];
+        for (size_t k = 0; k < t.coef.size(); ++k) coef_[(size_t)(coOff_[i] + (int)k) * V + l] = t.coef[k];
+        for (size_t k = 0; k < t.state.size(); ++k) state_[(size_t)(stOff_[i] + (int)k) * V + l] = t.state[k];
+      }
+    }
+    commit();
+  }
+  void commit()
+  {
+    check(mlb_graph_set_coefs(g_, coef_.data()));
+    check(mlb_graph_set_state(g_, state_.data()));
+  }
+  int instruments() const { return instruments_; }
+  const char* kernelName() const { return g_ ? mlb_graph_kernel_name(g_) : ""; }
+
+  // per-instrument, per-voice value of a tr::param(name, ...) scalar; call commit() after a batch of changes
+  void setParam(const std::string& name, int instrument, int voice, float value)
+  {
+    if (!g_) throw Error(MLB_ERR_INVALID, "mlb::tr::TracedSynth: compile() first");
+    if (instrument < 0 || instrument >= instruments_ || voice < 0 || voice >= numVoices_)
+      throw Error(MLB_ERR_INVALID, "mlb::tr::TracedSynth: no such instrument or voice");
+    for (size_t i = 0; i < nodes_.size(); ++i)
+      if (voices_[0].nodes[i].name == name)
+      {
+        coef_[(size_t)coOff_[i] * instruments_ * lanesPer_ + lane(instrument, voice)] = value;
+        return;
+      }
+    throw Error(MLB_ERR_INVALID, ("mlb::tr::TracedSynth: no param named " + name).c_str());
+  }
+
+  // nBlocks vectors of every instrument: raw events (offsets [nBlocks][instruments + 1] into events, times 0..63 in
+  // the vector) and, if processVoice reads the beat phase, host transport updates (timeOffsets [nBlocks][instruments + 1]
+  // into transports) in; bus [nBlocks][outputs][instruments][64] out -- what each instrument's Synth::processVector
+  // writes to its outputs.  Routing, Voice rows, controllers, beat phase, graph and bus sum run on the device
+  // (mlb_synth_process_context_host); state carries over from call to call.
+  void process(const int32_t* offsets, const mlb_event* events, int nEvents, const int32_t* timeOffsets,
+               const mlb_transport* transports, int nTransports, float* bus, int nBlocks)
+  {
+    if (!g_) throw Error(MLB_ERR_INVALID, "mlb::tr::TracedSynth: compile() first");
+    check(mlb_synth_process_context_host(routers_->handle(), voiceBank_->handle(), ctrl_ ? ctrl_->handle() : nullptr,
+                                         times_ ? times_->handle() : nullptr, g_, buses_->handle(), offsets, events,
+                                         nEvents, times_ ? timeOffsets : nullptr, times_ ? transports : nullptr,
+                                         times_ ? nTransports : 0, nullptr, nullptr, bus, nBlocks));
+    // A voice's record holds MLB_VOICE_MAX_EVENTS note events per vector (in unison every note event goes to every
+    // voice); the router drops and counts the rest, where the reference's Voice would have written them all.
+    std::vector<int64_t> overflow((size_t)instruments_);
+    routers_->counters(overflow.data(), nullptr);
+    overflow.swap(overflow_);
+    for (int g = 0; g < instruments_; ++g)
+      if (overflow[(size_t)g] != overflow_[(size_t)g])
+        throw Error(MLB_ERR_UNSUPPORTED,
+                    ("mlb::tr::TracedSynth: instrument " + std::to_string(g) + ": " +
+                     std::to_string(overflow_[(size_t)g] - overflow[(size_t)g]) +
+                     " note events found their voice's record full (" + std::to_string(MLB_VOICE_MAX_EVENTS) +
+                     " per voice and vector) and were dropped; this call's bus rows differ from the reference")
+                        .c_str());
+  }
 };
 
 }  // namespace tr
