@@ -595,16 +595,19 @@ class DeviceBank
   int n_out_ = 0;
 
  public:
-  DeviceBank(const Graph& graph, int rows, unsigned flags = MLB_GRAPH_EXACT) : rows_(rows)
+  DeviceBank(const Graph& graph, int rows, unsigned flags = MLB_GRAPH_EXACT)
+      : DeviceBank(graph.nodes(), graph.outs(), rows, flags)
   {
-    const auto& n = graph.nodes();
-    st_off_.resize(n.size());
-    co_off_.resize(n.size());
-    check(mlb_graph_layout(n.data(), (int)n.size(), &layout_, st_off_.data(), co_off_.data()));
-    check(mlb_graph_create(n.data(), (int)n.size(), graph.outs().data(), (int)graph.outs().size(), rows, flags, &g_));
+  }
+  DeviceBank(const std::vector<mlb_node>& nodes, const std::vector<int32_t>& outs, int rows, unsigned flags) : rows_(rows)
+  {
+    st_off_.resize(nodes.size());
+    co_off_.resize(nodes.size());
+    check(mlb_graph_layout(nodes.data(), (int)nodes.size(), &layout_, st_off_.data(), co_off_.data()));
+    check(mlb_graph_create(nodes.data(), (int)nodes.size(), outs.data(), (int)outs.size(), rows, flags, &g_));
     coef_.assign((size_t)layout_.n_coef_words * rows, 0.f);
     state_.assign((size_t)layout_.n_state_words * rows, 0u);
-    n_out_ = (int)graph.outs().size();
+    n_out_ = (int)outs.size();
   }
   ~DeviceBank() { mlb_graph_destroy(g_); }
   DeviceBank(const DeviceBank&) = delete;
@@ -617,9 +620,10 @@ class DeviceBank
   // like assigning `bank[row].coeffs = T::makeCoeffs(...)` in the reference
   void setCoeffs(int node, int row, const float* c, int n)
   {
-    for (int k = 0; k < n; ++k) coef_[(size_t)(co_off_[node] + k) * rows_ + row] = c[k];
+    for (int k = 0; k < n; ++k) setCoef(node, k, row, c[k]);
   }
   void setParam(int node, int row, float v) { setCoeffs(node, row, &v, 1); }
+  void setCoef(int node, int word, int row, float v) { coef_[(size_t)(co_off_[node] + word) * rows_ + row] = v; }
   void setStateWord(int node, int slot, int row, uint32_t w) { state_[(size_t)(st_off_[node] + slot) * rows_ + row] = w; }
   void commit()  // upload coefficients and state
   {

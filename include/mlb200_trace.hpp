@@ -71,6 +71,12 @@ struct TNode
   std::string name;             // named PARAMs
 };
 
+// a further call of an earlier functor (MLB_AGAIN): it owns no words of its own
+inline bool isAgain(const mlb_node& n)
+{
+  return n.iarg < 0 && n.op != MLB_OP_INPUT && n.op != MLB_OP_PARAM && n.op != MLB_OP_FEEDBACK_WRITE;
+}
+
 class Recorder
 {
  public:
@@ -148,6 +154,17 @@ class Recorder
     }
     nodes.push_back(t);
     return (int)nodes.size() - 1;
+  }
+  // After the second pass: the expression a stale symbol stood for is, in this pass, the node with the same operation
+  // index; it is written back at the end of the block.  `fn` names the traced function in the error.
+  void closeFeedback(const std::string& fn)
+  {
+    for (const auto& fr : feedbackReaders)
+    {
+      auto it = opIndexToNode.find(fr.first);
+      if (it == opIndexToNode.end()) throw Error(MLB_ERR_INVALID, ("mlb::tr: " + fn + " is not deterministic between calls").c_str());
+      addNode(MLB_OP_FEEDBACK_WRITE, {it->second}, fr.second, false);
+    }
   }
 };
 
@@ -1568,6 +1585,58 @@ class Synth : public SignalProcessor
 };
 
 // ------------------------------------------------------------------------------------------------------
+// what TracedProcessor and TracedSynth share
+
+// Records into `rec` for the lifetime of the scope.  On exit, normal or thrown, the recorder stops, the previous one
+// is current again and the context no longer answers for a synth voice.
+class TraceScope
+{
+  Recorder& rec_;
+  Recorder* prev_;
+  AudioContext& ctx_;
+
+ public:
+  TraceScope(Recorder& rec, AudioContext& ctx) : rec_(rec), prev_(Recorder::current()), ctx_(ctx) { Recorder::current() = &rec; }
+  ~TraceScope()
+  {
+    rec_.active = false;
+    Recorder::current() = prev_;
+    ctx_.pass_ = nullptr;
+  }
+  TraceScope(const TraceScope&) = delete;
+  TraceScope& operator=(const TraceScope&) = delete;
+};
+
+// Lay the traced graph out once at trace time: that is where a functor with a delay ring that is called again is
+// refused.  The bank lays it out again when it is compiled.
+inline void checkLayout(const std::vector<mlb_node>& nodes)
+{
+  mlb_layout layout;
+  check(mlb_graph_layout(nodes.data(), (int)nodes.size(), &layout, nullptr, nullptr));
+}
+
+// the initial coefficient and state words of traced node `node` into one row of the bank
+inline void loadWords(DeviceBank& bank, int node, int row, const TNode& t)
+{
+  if (isAgain(t.node)) return;  // the words belong to the functor's first call
+  for (size_t k = 0; k < t.coef.size(); ++k) bank.setCoef(node, (int)k, row, t.coef[k]);
+  for (size_t k = 0; k < t.state.size(); ++k) bank.setStateWord(node, (int)k, row, t.state[k]);
+}
+
+// coefficient or state words as a JSON list body of decimal bit patterns: an exact round trip
+template <class Word>
+inline void printWords(FILE* f, const std::vector<Word>& words)
+{
+  static_assert(sizeof(Word) == 4, "32-bit words");
+  for (size_t k = 0; k < words.size(); ++k)
+  {
+    uint32_t u;
+    std::memcpy(&u, &words[k], 4);
+    std::fprintf(f, "%s%u", k ? ", " : "", u);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------
 // TracedProcessor: trace a SignalProcessFn, compile it for `instances` independent copies, run it on the GPU.
 
 class TracedProcessor
@@ -1575,15 +1644,16 @@ class TracedProcessor
   Recorder rec_;
   std::vector<mlb_node> nodes_;
   std::vector<int32_t> outs_;
-  std::vector<int32_t> stOff_, coOff_;
-  mlb_layout layout_{};
-  std::vector<float> coef_;
-  std::vector<uint32_t> state_;
   std::map<std::string, int> named_;
-  mlb_graph* g_ = nullptr;
-  int instances_ = 0;
+  std::unique_ptr<DeviceBank> bank_;
   size_t nIn_ = 0, nOut_ = 0;
-  BatchedSignalProcessBuffer* buffer_ = nullptr;
+  std::unique_ptr<BatchedSignalProcessBuffer> buffer_;
+
+  DeviceBank& bank() const
+  {
+    if (!bank_) throw Error(MLB_ERR_INVALID, "mlb::tr: compile() first");
+    return *bank_;
+  }
 
   void runPass(AudioContext* ctx, SignalProcessFn fn, void* state)
   {
@@ -1595,50 +1665,25 @@ class TracedProcessor
 
  public:
   TracedProcessor() = default;
-  ~TracedProcessor()
-  {
-    if (g_) mlb_graph_destroy(g_);
-    delete buffer_;
-  }
   TracedProcessor(const TracedProcessor&) = delete;
   TracedProcessor& operator=(const TracedProcessor&) = delete;
 
   // Record the graph `fn` builds (host only: works without a GPU).
   void trace(AudioContext* ctx, SignalProcessFn fn, void* state)
   {
-    Recorder*& cur = Recorder::current();
-    Recorder* prev = cur;
-    cur = &rec_;
-    try
     {
+      TraceScope scope(rec_, *ctx);
       runPass(ctx, fn, state);  // pass 1: discovers which symbols survive the call
       runPass(ctx, fn, state);  // pass 2: the graph; stale symbols of pass 1 become feedback edges
-      // the expression a stale symbol stood for is, in this pass, the node with the same operation index
-      for (const auto& fr : rec_.feedbackReaders)
-      {
-        auto it = rec_.opIndexToNode.find(fr.first);
-        if (it == rec_.opIndexToNode.end()) throw Error(MLB_ERR_INVALID, "mlb::tr: process function is not deterministic between calls");
-        const int w = rec_.addNode(MLB_OP_FEEDBACK_WRITE, {it->second}, fr.second, false);
-        (void)w;
-      }
+      rec_.closeFeedback("process function");
       nOut_ = ctx->outputs.size();
       for (size_t i = 0; i < nOut_; ++i) rec_.outs.push_back(ctx->outputs[i].resolve());
     }
-    catch (...)
-    {
-      rec_.active = false;
-      cur = prev;
-      throw;
-    }
-    rec_.active = false;
-    cur = prev;
     nIn_ = ctx->inputs.size();
     nodes_.clear();
     for (const TNode& t : rec_.nodes) nodes_.push_back(t.node);
     outs_.assign(rec_.outs.begin(), rec_.outs.end());
-    stOff_.assign(nodes_.size(), 0);
-    coOff_.assign(nodes_.size(), 0);
-    check(mlb_graph_layout(nodes_.data(), (int)nodes_.size(), &layout_, stOff_.data(), coOff_.data()));
+    checkLayout(nodes_);
     named_.clear();
     for (size_t i = 0; i < rec_.nodes.size(); ++i)
       if (!rec_.nodes[i].name.empty()) named_[rec_.nodes[i].name] = (int)i;
@@ -1650,10 +1695,6 @@ class TracedProcessor
   size_t inputs() const { return nIn_; }
   size_t outputs() const { return nOut_; }
 
-  static bool isAgain(const mlb_node& n)
-  {
-    return n.iarg < 0 && n.op != MLB_OP_INPUT && n.op != MLB_OP_PARAM && n.op != MLB_OP_FEEDBACK_WRITE;
-  }
   // Write the traced graph as JSON (nodes, outs, initial coefficient and state words): lets a test or a tool
   // rebuild it elsewhere (tests/test_trace.py feeds it to the CPU checkers).
   void dump(FILE* f) const
@@ -1665,15 +1706,10 @@ class TracedProcessor
       std::fprintf(f, "%s{\"op\": %d, \"in\": [", i ? ", " : "", t.node.op);
       for (int k = 0; k < MLB_MAX_INS; ++k) std::fprintf(f, "%s%d", k ? ", " : "", t.node.in[k]);
       std::fprintf(f, "], \"iarg\": %d, \"coef\": [", t.node.iarg);
-      const bool again = isAgain(t.node);  // a further call of an earlier functor owns no words
-      for (size_t k = 0; k < t.coef.size() && !again; ++k)
-      {
-        uint32_t u;
-        std::memcpy(&u, &t.coef[k], 4);
-        std::fprintf(f, "%s%u", k ? ", " : "", u);  // bit patterns: exact round trip
-      }
+      const bool again = isAgain(t.node);
+      if (!again) printWords(f, t.coef);
       std::fprintf(f, "], \"state\": [");
-      for (size_t k = 0; k < t.state.size() && !again; ++k) std::fprintf(f, "%s%u", k ? ", " : "", t.state[k]);
+      if (!again) printWords(f, t.state);
       std::fprintf(f, "], \"name\": \"%s\"}", t.name.c_str());
     }
     std::fprintf(f, "], \"outs\": [");
@@ -1685,43 +1721,29 @@ class TracedProcessor
   void compile(int instances, unsigned flags = MLB_GRAPH_EXACT)
   {
     if (nodes_.empty()) throw Error(MLB_ERR_INVALID, "mlb::tr: trace() first");
-    if (g_) mlb_graph_destroy(g_), g_ = nullptr;
-    instances_ = instances;
-    check(mlb_graph_create(nodes_.data(), (int)nodes_.size(), outs_.data(), (int)outs_.size(), instances, flags, &g_));
-    coef_.assign((size_t)layout_.n_coef_words * instances, 0.f);
-    state_.assign((size_t)layout_.n_state_words * instances, 0u);
+    bank_.reset();  // the old graph's device memory is freed before the new graph's is allocated
+    bank_.reset(new DeviceBank(nodes_, outs_, instances, flags));
     for (size_t i = 0; i < rec_.nodes.size(); ++i)
-    {
-      const TNode& t = rec_.nodes[i];
-      if (isAgain(t.node)) continue;  // the words belong to the functor's first call
-      for (size_t k = 0; k < t.coef.size(); ++k)
-        for (int v = 0; v < instances; ++v) coef_[(size_t)(coOff_[i] + (int)k) * instances + v] = t.coef[k];
-      for (size_t k = 0; k < t.state.size(); ++k)
-        for (int v = 0; v < instances; ++v) state_[(size_t)(stOff_[i] + (int)k) * instances + v] = t.state[k];
-    }
+      for (int v = 0; v < instances; ++v) loadWords(*bank_, (int)i, v, rec_.nodes[i]);
     commit();
   }
-  void commit()
-  {
-    check(mlb_graph_set_coefs(g_, coef_.data()));
-    check(mlb_graph_set_state(g_, state_.data()));
-  }
-  int instances() const { return instances_; }
-  const char* kernelName() const { return g_ ? mlb_graph_kernel_name(g_) : ""; }
+  void commit() { bank().commit(); }
+  int instances() const { return bank_ ? bank_->rows() : 0; }
+  const char* kernelName() const { return bank_ ? bank_->kernelName() : ""; }
   // per-instance value of a tr::param(name, ...) scalar; call commit() after a batch of changes
   void setParam(const std::string& name, int instance, float value)
   {
     auto it = named_.find(name);
     if (it == named_.end()) throw Error(MLB_ERR_INVALID, "mlb::tr: no such param");
-    coef_[(size_t)coOff_[(size_t)it->second] * instances_ + instance] = value;
+    bank().setParam(it->second, instance, value);
   }
   // per-instance coefficient / state word of node `node` (indices as in nodes())
-  void setCoef(int node, int word, int instance, float value) { coef_[(size_t)(coOff_[(size_t)node] + word) * instances_ + instance] = value; }
-  void setStateWord(int node, int word, int instance, uint32_t value) { state_[(size_t)(stOff_[(size_t)node] + word) * instances_ + instance] = value; }
+  void setCoef(int node, int word, int instance, float value) { bank().setCoef(node, word, instance, value); }
+  void setStateWord(int node, int word, int instance, uint32_t value) { bank().setStateWord(node, word, instance, value); }
 
   // n_blocks successive process calls for every instance in ONE kernel launch.
   // in [T][inputs][instances][64], out [T][outputs][instances][64], mix [T][outputs][64] (sum over instances).
-  void processBlocks(const float* in, float* out, float* mix, int nBlocks) { check(mlb_graph_process_host(g_, in, out, mix, nBlocks)); }
+  void processBlocks(const float* in, float* out, float* mix, int nBlocks) { bank().process(in, out, mix, nBlocks); }
 
   // SignalProcessBuffer::process for ONE instance's I/O (source/app/MLSignalProcessBuffer.cpp:36-90): any host
   // buffer size; every vector the callback needs is computed by one launch.  With instances > 1 the outputs are
@@ -1729,25 +1751,26 @@ class TracedProcessor
   // instance receives the same external inputs.
   void process(const float** externalInputs, float** externalOutputs, int nFrames, int maxFrames = 4096)
   {
-    if (!g_) throw Error(MLB_ERR_INVALID, "mlb::tr: compile() first");
-    if (!buffer_) buffer_ = new BatchedSignalProcessBuffer(nIn_, nOut_, (size_t)maxFrames);
+    DeviceBank& bank = this->bank();
+    if (!buffer_) buffer_.reset(new BatchedSignalProcessBuffer(nIn_, nOut_, (size_t)maxFrames));
     std::vector<float>& bin = bcast_;
+    const int instances = bank.rows();
     buffer_->process(externalInputs, externalOutputs, nFrames,
                      [&](const float* in, float* out, int nVec)
                      {
                        const float* src = in;
-                       if (nIn_ && instances_ > 1)
+                       if (nIn_ && instances > 1)
                        {
-                         bin.resize((size_t)nVec * nIn_ * instances_ * MLB_BLOCK);
+                         bin.resize((size_t)nVec * nIn_ * instances * MLB_BLOCK);
                          for (size_t r = 0; r < (size_t)nVec * nIn_; ++r)
-                           for (int v = 0; v < instances_; ++v)
-                             std::memcpy(&bin[(r * instances_ + v) * MLB_BLOCK], in + r * MLB_BLOCK, MLB_BLOCK * 4);
+                           for (int v = 0; v < instances; ++v)
+                             std::memcpy(&bin[(r * instances + v) * MLB_BLOCK], in + r * MLB_BLOCK, MLB_BLOCK * 4);
                          src = bin.data();
                        }
-                       if (instances_ > 1)
-                         check(mlb_graph_process_host(g_, nIn_ ? src : nullptr, nullptr, out, nVec));
+                       if (instances > 1)
+                         bank.process(nIn_ ? src : nullptr, nullptr, out, nVec);
                        else
-                         check(mlb_graph_process_host(g_, nIn_ ? src : nullptr, out, nullptr, nVec));
+                         bank.process(nIn_ ? src : nullptr, out, nullptr, nVec);
                      });
   }
 
@@ -1774,8 +1797,7 @@ class TracedSynth
   };
   std::vector<VoiceGraph> voices_;  // one per synth voice
   std::vector<mlb_node> nodes_;
-  std::vector<int32_t> outs_, stOff_, coOff_;
-  mlb_layout layout_{};
+  std::vector<int32_t> outs_;
   std::vector<int> controllers_;
   bool phase_ = false;
   AudioContext::InputSettings settings_;
@@ -1784,15 +1806,19 @@ class TracedSynth
   size_t nOut_ = 0;
 
   int instruments_ = 0, lanesPer_ = 0;
-  std::vector<float> coef_;
-  std::vector<uint32_t> state_;
-  mlb_graph* g_ = nullptr;
   std::unique_ptr<RouterBank> routers_;
   std::unique_ptr<VoiceBank> voiceBank_;
   std::unique_ptr<ControllerBank> ctrl_;
   std::unique_ptr<ProcessTimeBank> times_;
   std::unique_ptr<Buses> buses_;
+  std::unique_ptr<DeviceBank> bank_;  // the graph over every lane
   std::vector<int64_t> overflow_;  // the router bank's overflow counts after the last call
+
+  DeviceBank& bank() const
+  {
+    if (!bank_) throw Error(MLB_ERR_INVALID, "mlb::tr::TracedSynth: compile() first");
+    return *bank_;
+  }
 
   [[noreturn]] static void refuse(int v, const std::string& what)
   {
@@ -1865,7 +1891,7 @@ class TracedSynth
       for (int k = 0; k < MLB_MAX_INS; ++k)
         if (t.node.in[k] >= 0) t.node.in[k] = idx[(size_t)t.node.in[k]];
       if (t.node.op == MLB_OP_FEEDBACK_WRITE) t.node.iarg = idx[(size_t)t.node.iarg];
-      else if (TracedProcessor::isAgain(t.node)) t.node.iarg = MLB_AGAIN(idx[(size_t)MLB_AGAIN_TARGET(t.node.iarg)]);
+      else if (isAgain(t.node)) t.node.iarg = MLB_AGAIN(idx[(size_t)MLB_AGAIN_TARGET(t.node.iarg)]);
     }
     for (int i = 0; i < nOut; ++i) vg.outs.push_back(x[(size_t)i] < 0 ? -1 : idx[(size_t)x[(size_t)i]]);
     return vg;
@@ -1895,10 +1921,6 @@ class TracedSynth
 
  public:
   TracedSynth() = default;
-  ~TracedSynth()
-  {
-    if (g_) mlb_graph_destroy(g_);
-  }
   TracedSynth(const TracedSynth&) = delete;
   TracedSynth& operator=(const TracedSynth&) = delete;
 
@@ -1931,12 +1953,9 @@ class TracedSynth
     bool phase = false;
     std::vector<VoiceGraph> graphs;
     std::vector<SynthPass> passes((size_t)V);  // kept for the whole trace: a Voice& held by a later voice stays valid
-    Recorder*& cur = Recorder::current();
-    Recorder* prev = cur;
-    cur = &rec;
-    rec.functorVoice = &functorVoice;
-    try
     {
+      TraceScope scope(rec, ctx);
+      rec.functorVoice = &functorVoice;
       for (int v = 0; v < V; ++v)
       {
         SynthPass& pass = passes[(size_t)v];
@@ -1964,12 +1983,7 @@ class TracedSynth
           synth.processVoice(v, ctx.getInputVoice(v), ctx.inputs, ctx.outputs, &ctx);
           ctx.pass_ = nullptr;
         }
-        for (const auto& fr : rec.feedbackReaders)
-        {
-          auto it = rec.opIndexToNode.find(fr.first);
-          if (it == rec.opIndexToNode.end()) throw Error(MLB_ERR_INVALID, "mlb::tr: processVoice is not deterministic between calls");
-          rec.addNode(MLB_OP_FEEDBACK_WRITE, {it->second}, fr.second, false);
-        }
+        rec.closeFeedback("processVoice");
         fin.clear();
         for (size_t i = 0; i < ctx.outputs.size(); ++i) fin.push_back(ctx.outputs[i].resolve());
         phase = phase || pass.phaseNode >= 0;
@@ -1980,15 +1994,6 @@ class TracedSynth
                         "); voices may differ in coefficients and state only");
       }
     }
-    catch (...)
-    {
-      ctx.pass_ = nullptr;
-      rec.active = false;
-      cur = prev;
-      throw;
-    }
-    rec.active = false;
-    cur = prev;
     // the beat phase after the controllers; untouched outputs read one shared +0 row
     const int phasePlane = MLB_VOICE_ROWS + (int)controllers.size();
     for (VoiceGraph& vg : graphs)
@@ -2022,9 +2027,7 @@ class TracedSynth
     nodes_.clear();
     for (const TNode& t : voices_[0].nodes) nodes_.push_back(t.node);
     outs_ = voices_[0].outs;
-    stOff_.assign(nodes_.size(), 0);
-    coOff_.assign(nodes_.size(), 0);
-    check(mlb_graph_layout(nodes_.data(), (int)nodes_.size(), &layout_, stOff_.data(), coOff_.data()));
+    checkLayout(nodes_);
   }
 
   const std::vector<mlb_node>& nodes() const { return nodes_; }
@@ -2054,25 +2057,18 @@ class TracedSynth
       std::fprintf(f, "%s{\"op\": %d, \"in\": [", i ? ", " : "", m.op);
       for (int k = 0; k < MLB_MAX_INS; ++k) std::fprintf(f, "%s%d", k ? ", " : "", m.in[k]);
       std::fprintf(f, "], \"iarg\": %d, \"name\": \"%s\", \"coef\": [", m.iarg, voices_[0].nodes[i].name.c_str());
-      const bool again = TracedProcessor::isAgain(m);  // a further call of an earlier functor owns no words
+      const bool again = isAgain(m);
       for (size_t v = 0; v < voices_.size(); ++v)
       {
-        const TNode& t = voices_[v].nodes[i];
         std::fprintf(f, "%s[", v ? ", " : "");
-        for (size_t k = 0; k < t.coef.size() && !again; ++k)
-        {
-          uint32_t u;
-          std::memcpy(&u, &t.coef[k], 4);
-          std::fprintf(f, "%s%u", k ? ", " : "", u);
-        }
+        if (!again) printWords(f, voices_[v].nodes[i].coef);
         std::fprintf(f, "]");
       }
       std::fprintf(f, "], \"state\": [");
       for (size_t v = 0; v < voices_.size(); ++v)
       {
-        const TNode& t = voices_[v].nodes[i];
         std::fprintf(f, "%s[", v ? ", " : "");
-        for (size_t k = 0; k < t.state.size() && !again; ++k) std::fprintf(f, "%s%u", k ? ", " : "", t.state[k]);
+        if (!again) printWords(f, voices_[v].nodes[i].state);
         std::fprintf(f, "]");
       }
       std::fprintf(f, "]}");
@@ -2089,8 +2085,7 @@ class TracedSynth
   {
     if (nodes_.empty()) throw Error(MLB_ERR_INVALID, "mlb::tr::TracedSynth: trace() first");
     if (instruments < 1) throw Error(MLB_ERR_INVALID, "mlb::tr::TracedSynth: instruments must be positive");
-    if (g_) mlb_graph_destroy(g_), g_ = nullptr;
-    buses_.reset(), times_.reset(), ctrl_.reset(), voiceBank_.reset(), routers_.reset();
+    bank_.reset(), buses_.reset(), times_.reset(), ctrl_.reset(), voiceBank_.reset(), routers_.reset();
     const AudioContext::InputSettings& s = settings_;
     const int G = instruments, NR = lanesPerInstrument(), V = G * NR;
     instruments_ = G, lanesPer_ = NR;
@@ -2123,41 +2118,27 @@ class TracedSynth
       times_.reset(new ProcessTimeBank(G, sampleRate_));
       times_->setVoiceMap(inst.data(), V);
     }
-    check(mlb_graph_create(nodes_.data(), (int)nodes_.size(), outs_.data(), (int)outs_.size(), V, flags, &g_));
+    bank_.reset(new DeviceBank(nodes_, outs_, V, flags));
     buses_.reset(new Buses(V, G, busFirst.data(), busCount.data()));
     overflow_.assign((size_t)G, 0);
-    coef_.assign((size_t)layout_.n_coef_words * V, 0.f);
-    state_.assign((size_t)layout_.n_state_words * V, 0u);
     for (size_t i = 0; i < nodes_.size(); ++i)
-    {
-      if (TracedProcessor::isAgain(nodes_[i])) continue;  // the words belong to the functor's first call
-      for (int l = 0; l < V; ++l)
-      {
-        const TNode& t = voices_[(size_t)laneVoice(l % NR)].nodes[i];
-        for (size_t k = 0; k < t.coef.size(); ++k) coef_[(size_t)(coOff_[i] + (int)k) * V + l] = t.coef[k];
-        for (size_t k = 0; k < t.state.size(); ++k) state_[(size_t)(stOff_[i] + (int)k) * V + l] = t.state[k];
-      }
-    }
+      for (int l = 0; l < V; ++l) loadWords(*bank_, (int)i, l, voices_[(size_t)laneVoice(l % NR)].nodes[i]);
     commit();
   }
-  void commit()
-  {
-    check(mlb_graph_set_coefs(g_, coef_.data()));
-    check(mlb_graph_set_state(g_, state_.data()));
-  }
+  void commit() { bank().commit(); }
   int instruments() const { return instruments_; }
-  const char* kernelName() const { return g_ ? mlb_graph_kernel_name(g_) : ""; }
+  const char* kernelName() const { return bank_ ? bank_->kernelName() : ""; }
 
   // per-instrument, per-voice value of a tr::param(name, ...) scalar; call commit() after a batch of changes
   void setParam(const std::string& name, int instrument, int voice, float value)
   {
-    if (!g_) throw Error(MLB_ERR_INVALID, "mlb::tr::TracedSynth: compile() first");
+    DeviceBank& bank = this->bank();
     if (instrument < 0 || instrument >= instruments_ || voice < 0 || voice >= numVoices_)
       throw Error(MLB_ERR_INVALID, "mlb::tr::TracedSynth: no such instrument or voice");
     for (size_t i = 0; i < nodes_.size(); ++i)
       if (voices_[0].nodes[i].name == name)
       {
-        coef_[(size_t)coOff_[i] * instruments_ * lanesPer_ + lane(instrument, voice)] = value;
+        bank.setParam((int)i, lane(instrument, voice), value);
         return;
       }
     throw Error(MLB_ERR_INVALID, ("mlb::tr::TracedSynth: no param named " + name).c_str());
@@ -2171,9 +2152,9 @@ class TracedSynth
   void process(const int32_t* offsets, const mlb_event* events, int nEvents, const int32_t* timeOffsets,
                const mlb_transport* transports, int nTransports, float* bus, int nBlocks)
   {
-    if (!g_) throw Error(MLB_ERR_INVALID, "mlb::tr::TracedSynth: compile() first");
+    mlb_graph* graph = bank().handle();
     check(mlb_synth_process_context_host(routers_->handle(), voiceBank_->handle(), ctrl_ ? ctrl_->handle() : nullptr,
-                                         times_ ? times_->handle() : nullptr, g_, buses_->handle(), offsets, events,
+                                         times_ ? times_->handle() : nullptr, graph, buses_->handle(), offsets, events,
                                          nEvents, times_ ? timeOffsets : nullptr, times_ ? transports : nullptr,
                                          times_ ? nTransports : 0, nullptr, nullptr, bus, nBlocks));
     // A voice's record holds MLB_VOICE_MAX_EVENTS note events per vector (in unison every note event goes to every
