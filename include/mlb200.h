@@ -801,6 +801,65 @@ int mlb_synth_process_context_host(mlb_routers* r, mlb_voices* vb, mlb_controlle
                                    int n_events, const int32_t* time_offsets_host, const mlb_transport* transports_host,
                                    int n_transports, float* out_host, float* mix_host, float* bus_host, int n_blocks);
 
+/* ---- Published signals of G instruments (K14) --------------------------------------------------
+ * A synth calls publishSignal(name, maxFrames, maxVoices, channels, octavesDown) in its setup and
+ * storePublishedSignal(name, DSPVectorArray<channels>, frames, voice) in processVoice; a UI reads the signal with
+ * getPublishedSignals()[name]->readLatest(...) (SignalProcessor::PublishedSignal, MLSignalProcessor.h:28-105,
+ * .cpp:11-38).  A published bank holds that state for G instruments: per instrument and signal a ring of
+ * max(2^bitsToContain(max_frames * channels * max_voices), 64) floats with its read and write index, and one
+ * decimation counter shared by the instrument's voices.  Its input is the graph's published planes: each store item,
+ * in call order within processVoice, owns `channels` consecutive planes, item 0 first.  Per vector the stores arrive
+ * in voice order (voices first_voice[g] .. + voice_count[g] of instrument g), then in call order, and every
+ * 2^octaves_down-th frame of that sequence is written, its channels side by side -- the reference's writeQuick calls,
+ * bit for bit, across vectors and calls.  Rings, indices and counters are the reference's, clobbering included. */
+#define MLB_PUBLISHED_MAX_SIGNALS 16
+#define MLB_PUBLISHED_MAX_STORES 64
+typedef struct mlb_published_signal {
+  int32_t max_frames;    /* the frames of one store at most (1..64 is useful; every store must fit) */
+  int32_t max_voices;    /* >= 1: sizes the ring, as in the reference */
+  int32_t channels;      /* 1..64 */
+  int32_t octaves_down;  /* 0..30: every 2^octaves_down-th frame is kept */
+} mlb_published_signal;
+typedef struct mlb_published_store {
+  int32_t signal;  /* index into the signals */
+  int32_t frames;  /* 0..64 and <= the signal's max_frames: the first `frames` frames of the vector */
+} mlb_published_store;
+enum { MLB_PUBLISHED_READ_LATEST = 0, /* PublishedSignal::readLatest: discard down to the request, then read */
+       MLB_PUBLISHED_READ = 1,        /* PublishedSignal::read: the oldest frames, consumed */
+       MLB_PUBLISHED_PEEK = 2,        /* PublishedSignal::peekLatest: the newest frames, nothing consumed; nothing is
+                                         copied when fewer are available */
+       MLB_PUBLISHED_AVAILABLE = 3 }; /* PublishedSignal::getAvailableFrames */
+typedef struct mlb_published mlb_published;
+/* Arguments are validated on the host; MLB_ERR_INVALID names the offending signal or store.  Rings start empty.
+ * A live bank counts toward mlb_init's one-device rule. */
+int mlb_published_create(int n_voices, int n_instruments, const int32_t* first_voice, const int32_t* voice_count,
+                         const mlb_published_signal* signals, int n_signals, const mlb_published_store* stores,
+                         int n_stores, mlb_published** out);
+int mlb_published_destroy(mlb_published* p);
+int mlb_published_clear(mlb_published* p);  /* every ring empty, every counter 0 */
+/* the published planes the graph's outputs end with: the sum of the stores' channels */
+int mlb_published_planes(const mlb_published* p);
+/* rows_dev [T][n_planes][V][64], the published planes at [plane0, plane0 + mlb_published_planes): one launch, no
+ * allocation, no synchronisation; nothing is launched when the bank has no store */
+int mlb_published_process_device(mlb_published* p, const float* rows_dev, int plane0, int n_planes, int n_blocks,
+                                 void* stream);
+/* One read of signal `signal` for every instrument (mode MLB_PUBLISHED_*): dest [G][frames * channels] (may be NULL for
+ * AVAILABLE), the part a read does not fill is zero; counts [G]: READ_LATEST and READ the floats read (the
+ * reference's return value), PEEK 1 when the newest frames were copied and 0 when fewer were available, AVAILABLE the
+ * available frames.  The device form is one launch on `stream`; the host form returns when its copies are finished. */
+int mlb_published_read_device(mlb_published* p, int signal, int mode, int frames, float* dest_dev, int32_t* counts_dev,
+                              void* stream);
+int mlb_published_read_host(mlb_published* p, int signal, int mode, int frames, float* dest_host, int32_t* counts_host);
+/* mlb_synth_process_context_host with buses and a published bank: per time chunk, after the graph, the bus sum reads
+ * the audio planes (the graph's first n_out - mlb_published_planes outputs) and K14 the published planes.  With a
+ * bank of no store this is mlb_synth_process_context_host.  MLB_ERR_INVALID also when the bank's voices differ from the
+ * graph's or the graph has no output besides the published planes. */
+int mlb_synth_process_published_host(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb, mlb_process_time* pt,
+                                     mlb_graph* g, mlb_buses* b, mlb_published* p, const int32_t* offsets_host,
+                                     const mlb_event* events_host, int n_events, const int32_t* time_offsets_host,
+                                     const mlb_transport* transports_host, int n_transports, float* bus_host,
+                                     int n_blocks);
+
 #ifdef __cplusplus
 }
 #endif

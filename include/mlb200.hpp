@@ -714,6 +714,42 @@ class Buses
   }
 };
 
+// Published signals of G instruments (mlb_published_*): the rings of SignalProcessor::PublishedSignal, written on the
+// device from the graph's published planes, read for every instrument in one call.
+class PublishedBank
+{
+  mlb_published* p_ = nullptr;
+  int instruments_ = 0;
+  std::vector<mlb_published_signal> signals_;
+
+ public:
+  PublishedBank(int nVoices, int nInstruments, const int32_t* firstVoice, const int32_t* voiceCount,
+                const std::vector<mlb_published_signal>& signals, const std::vector<mlb_published_store>& stores)
+      : instruments_(nInstruments), signals_(signals)
+  {
+    check(mlb_published_create(nVoices, nInstruments, firstVoice, voiceCount, signals.data(), (int)signals.size(),
+                               stores.data(), (int)stores.size(), &p_));
+  }
+  ~PublishedBank() { mlb_published_destroy(p_); }
+  PublishedBank(const PublishedBank&) = delete;
+  PublishedBank& operator=(const PublishedBank&) = delete;
+  mlb_published* handle() const { return p_; }
+  int instruments() const { return instruments_; }
+  int planes() const { return mlb_published_planes(p_); }
+  int channels(int signal) const { return signals_.at((size_t)signal).channels; }
+  void clear() { check(mlb_published_clear(p_)); }
+  // one read of `signal` for every instrument (mode MLB_PUBLISHED_*): dest [instruments][frames * channels], counts
+  // [instruments]; host buffers
+  void read(int signal, int mode, int frames, float* dest, int32_t* counts)
+  {
+    check(mlb_published_read_host(p_, signal, mode, frames, dest, counts));
+  }
+  void readDevice(int signal, int mode, int frames, float* dest, int32_t* counts, void* stream = nullptr)
+  {
+    check(mlb_published_read_device(p_, signal, mode, frames, dest, counts, stream));
+  }
+};
+
 // processEvents with per-instrument output (mlb_synth_process_buses_host): events [nBlocks][voices] in,
 // bus [nBlocks][n_out][buses][64] out; the voice rows stay on the device.
 inline void processEventsToBuses(VoiceBank& voices, DeviceBank& bank, Buses& buses, const mlb_voice_events* events,

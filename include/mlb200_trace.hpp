@@ -1531,6 +1531,21 @@ class AudioContext
 };
 using SignalProcessFn = void (*)(AudioContext*, void*);
 
+using Path = std::string;  // the name of a published signal (the reference's ml::Path, made from a string)
+
+// A published signal as publishSignal declared it, and one storePublishedSignal call as TracedSynth::trace recorded it
+struct PublishDecl
+{
+  Path name;
+  int maxFrames, maxVoices, channels, octavesDown;
+};
+struct PublishStore
+{
+  int signal;             // index into the declarations
+  int frames;
+  std::vector<int> rows;  // the `channels` rows stored: node indices of the pass being recorded
+};
+
 // MLSignalProcessor.h: the base of Synth, reduced to what a Synth subclass uses
 class SignalProcessor
 {
@@ -1539,9 +1554,75 @@ class SignalProcessor
   virtual ~SignalProcessor() {}
   virtual void processVector(const DSPVectorDynamic& inputs, DSPVectorDynamic& outputs, void* stateData = nullptr) {}
   virtual void setSampleRate(double sr) { sampleRate_ = sr; }
+  const std::vector<PublishDecl>& publishedSignals() const { return published_; }
 
  protected:
   double sampleRate_{0};
+
+  // MLSignalProcessor.h:184-188: declares the signal (publishing a name again replaces its declaration)
+  void publishSignal(Path signalName, int maxFrames, int maxVoices, int channels, int octavesDown)
+  {
+    const std::string what = "mlb::tr: publishSignal(" + signalName + "): ";
+    if (maxFrames < 1 || maxVoices < 1 || channels < 1 || channels > (int)kFloatsPerDSPVector)
+      throw Error(MLB_ERR_UNSUPPORTED, (what + "maxFrames and maxVoices must be at least 1 and channels in 1..64").c_str());
+    if (octavesDown < 0 || octavesDown > 30)
+      throw Error(MLB_ERR_UNSUPPORTED, (what + "octavesDown " + std::to_string(octavesDown) + " is not in 0..30").c_str());
+    for (PublishDecl& d : published_)
+      if (d.name == signalName)
+      {
+        d = PublishDecl{signalName, maxFrames, maxVoices, channels, octavesDown};
+        return;
+      }
+    published_.push_back(PublishDecl{signalName, maxFrames, maxVoices, channels, octavesDown});
+  }
+
+  // MLSignalProcessor.h:193-201: inside TracedSynth::trace, records the rows as graph outputs of the voice; a name that
+  // was never published stores nothing, as in the reference
+  template <size_t CHANNELS>
+  void storePublishedSignal(Path signalName, const DSPVectorArray<CHANNELS>& inputVec, int frames, int voice)
+  {
+    (void)voice;
+    int s = 0;
+    while (s < (int)published_.size() && published_[(size_t)s].name != signalName) ++s;
+    if (s == (int)published_.size()) return;
+    const PublishDecl& d = published_[(size_t)s];
+    const std::string what = "mlb::tr: storePublishedSignal(" + signalName + "): ";
+    if (!publishStores_) throw Error(MLB_ERR_INVALID, (what + "outside TracedSynth::trace()").c_str());
+    if ((int)CHANNELS != d.channels)
+      throw Error(MLB_ERR_UNSUPPORTED, (what + "a DSPVectorArray<" + std::to_string(CHANNELS) + "> into a signal of " +
+                                        std::to_string(d.channels) + " channels (the reference's rotate buffer would be "
+                                        "mis-sized)").c_str());
+    if (frames < 0 || frames > (int)kFloatsPerDSPVector)
+      throw Error(MLB_ERR_UNSUPPORTED, (what + "frames " + std::to_string(frames) + " is not in 0..64").c_str());
+    if (frames > d.maxFrames)
+      throw Error(MLB_ERR_UNSUPPORTED, (what + "frames " + std::to_string(frames) + " is above maxFrames " +
+                                        std::to_string(d.maxFrames) + " (the reference writes past its rotate buffer)")
+                                           .c_str());
+    PublishStore st{s, frames, {}};
+    for (size_t j = 0; j < CHANNELS; ++j) st.rows.push_back(inputVec.constRow((int)j).resolve());
+    publishStores_->push_back(st);
+  }
+  // one row: the reference's DSPVector is a DSPVectorArray<1>
+  void storePublishedSignal(Path signalName, const DSPVector& inputVec, int frames, int voice)
+  {
+    DSPVectorArray<1> a;
+    a.row(0) = inputVec;
+    storePublishedSignal(signalName, a, frames, voice);
+  }
+
+  // MLSignalProcessor.h:203-210: takes a host pointer, which has no symbolic form
+  void storePublishedSignalVert(Path signalName, const float*, int, int)
+  {
+    throw Error(MLB_ERR_UNSUPPORTED, ("mlb::tr: storePublishedSignalVert(" + signalName +
+                                      ") takes a host pointer and cannot be traced; store a DSPVectorArray with "
+                                      "storePublishedSignal")
+                                         .c_str());
+  }
+
+ private:
+  friend class TracedSynth;
+  std::vector<PublishDecl> published_;
+  std::vector<PublishStore>* publishStores_ = nullptr;  // set by TracedSynth::trace while processVoice runs
 };
 
 // Synth (MLSynth.h:26-93): subclasses implement processVoice; TracedSynth traces it once per voice
@@ -1794,10 +1875,13 @@ class TracedSynth
   {
     std::vector<TNode> nodes;
     std::vector<int32_t> outs;
+    std::vector<PublishStore> stores;  // rows: nodes of this graph
   };
   std::vector<VoiceGraph> voices_;  // one per synth voice
   std::vector<mlb_node> nodes_;
   std::vector<int32_t> outs_;
+  std::vector<PublishDecl> published_;  // the synth's publishSignal declarations
+  std::vector<int32_t> pubOuts_;        // graph outputs after outs_: the stored rows, store by store
   std::vector<int> controllers_;
   bool phase_ = false;
   AudioContext::InputSettings settings_;
@@ -1812,6 +1896,7 @@ class TracedSynth
   std::unique_ptr<ProcessTimeBank> times_;
   std::unique_ptr<Buses> buses_;
   std::unique_ptr<DeviceBank> bank_;  // the graph over every lane
+  std::unique_ptr<PublishedBank> pubBank_;
   std::vector<int64_t> overflow_;  // the router bank's overflow counts after the last call
 
   DeviceBank& bank() const
@@ -1825,8 +1910,10 @@ class TracedSynth
     throw Error(MLB_ERR_UNSUPPORTED, ("mlb::tr::TracedSynth: voice " + std::to_string(v) + " " + what).c_str());
   }
 
-  // the pass's graph without the accumulators and unread Voice rows; out i = x, or -1 for an untouched output
-  static VoiceGraph extract(const Recorder& rec, const std::vector<int>& acc, const std::vector<int>& fin, int v)
+  // the pass's graph without the accumulators and unread Voice rows; out i = x, or -1 for an untouched output; the
+  // stored rows of `stores` are kept and renumbered
+  static VoiceGraph extract(const Recorder& rec, const std::vector<int>& acc, const std::vector<int>& fin, int v,
+                            std::vector<PublishStore> stores)
   {
     const int n = (int)rec.nodes.size(), nOut = (int)acc.size();
     std::vector<char> drop((size_t)n, 0);
@@ -1877,6 +1964,13 @@ class TracedSynth
       if (drop[(size_t)s]) refuse(v, "adds one output into another");
       ++uses[(size_t)s];
     }
+    for (const PublishStore& st : stores)
+      for (int s : st.rows)
+      {
+        if (accOf[(size_t)s] >= 0) refuse(v, "publishes the accumulator " + name(accOf[(size_t)s]));
+        if (drop[(size_t)s]) refuse(v, "publishes an output after adding into it");
+        ++uses[(size_t)s];
+      }
     for (int j = 0; j < n; ++j)  // Voice rows the voice does not read
     {
       const mlb_node& m = rec.nodes[(size_t)j].node;
@@ -1894,6 +1988,9 @@ class TracedSynth
       else if (isAgain(t.node)) t.node.iarg = MLB_AGAIN(idx[(size_t)MLB_AGAIN_TARGET(t.node.iarg)]);
     }
     for (int i = 0; i < nOut; ++i) vg.outs.push_back(x[(size_t)i] < 0 ? -1 : idx[(size_t)x[(size_t)i]]);
+    for (PublishStore& st : stores)
+      for (int& s : st.rows) s = idx[(size_t)s];
+    vg.stores = std::move(stores);
     return vg;
   }
 
@@ -1901,6 +1998,11 @@ class TracedSynth
   {
     if (a.nodes.size() != b.nodes.size()) return where = "a different number of nodes", false;
     if (a.outs != b.outs) return where = "different outputs", false;
+    if (a.stores.size() != b.stores.size()) return where = "a different number of published stores", false;
+    for (size_t k = 0; k < a.stores.size(); ++k)
+      if (a.stores[k].signal != b.stores[k].signal || a.stores[k].frames != b.stores[k].frames ||
+          a.stores[k].rows != b.stores[k].rows)
+        return where = "published store " + std::to_string(k), false;
     for (size_t j = 0; j < a.nodes.size(); ++j)
     {
       const mlb_node &p = a.nodes[j].node, &q = b.nodes[j].node;
@@ -1953,8 +2055,15 @@ class TracedSynth
     bool phase = false;
     std::vector<VoiceGraph> graphs;
     std::vector<SynthPass> passes((size_t)V);  // kept for the whole trace: a Voice& held by a later voice stays valid
+    std::vector<PublishStore> stores;          // this pass's storePublishedSignal calls
     {
       TraceScope scope(rec, ctx);
+      struct StoreSink  // where the synth's stores are recorded, for the lifetime of the trace
+      {
+        SignalProcessor& sp;
+        ~StoreSink() { sp.publishStores_ = nullptr; }
+      } sink{synth};
+      synth.publishStores_ = &stores;
       rec.functorVoice = &functorVoice;
       for (int v = 0; v < V; ++v)
       {
@@ -1965,6 +2074,7 @@ class TracedSynth
         {
           rec.staleEpoch = p == 0 ? -2 : rec.epoch;  // pass 2 may read what pass 1 of this voice left
           rec.beginPass();
+          stores.clear();
           pass.voice = v;
           pass.controllers = &controllers;
           pass.controllerNode.clear();
@@ -1987,7 +2097,7 @@ class TracedSynth
         fin.clear();
         for (size_t i = 0; i < ctx.outputs.size(); ++i) fin.push_back(ctx.outputs[i].resolve());
         phase = phase || pass.phaseNode >= 0;
-        graphs.push_back(extract(rec, acc, fin, v));
+        graphs.push_back(extract(rec, acc, fin, v, stores));
         std::string where;
         if (v > 0 && !sameStructure(graphs[0], graphs.back(), where))
           refuse(v, "records a different graph from voice 0 (" + where +
@@ -2017,6 +2127,25 @@ class TracedSynth
           o = zero;
         }
     }
+    // every stored row leaves the graph through a copy of its own, select(x, x, x) (bitwise: exactly x), so that a row
+    // stored twice, stored and also added into an output, or a Voice row stored as it is, is one distinct output each
+    std::vector<int32_t> pubOuts;
+    for (VoiceGraph& vg : graphs)
+    {
+      pubOuts.clear();
+      for (const PublishStore& st : vg.stores)
+        for (int s : st.rows)
+        {
+          TNode c;
+          c.node.op = MLB_OP_SELECT;
+          for (int k = 0; k < MLB_MAX_INS; ++k) c.node.in[k] = k < 3 ? s : -1;
+          c.node.iarg = 0;
+          pubOuts.push_back((int32_t)vg.nodes.size());
+          vg.nodes.push_back(c);
+        }
+    }
+    published_ = synth.publishedSignals();
+    pubOuts_ = pubOuts;
     voices_ = std::move(graphs);
     controllers_ = controllers;
     phase_ = phase;
@@ -2033,6 +2162,9 @@ class TracedSynth
   const std::vector<mlb_node>& nodes() const { return nodes_; }
   const std::vector<int32_t>& outs() const { return outs_; }
   const std::vector<int>& controllers() const { return controllers_; }
+  const std::vector<PublishDecl>& published() const { return published_; }
+  const std::vector<PublishStore>& stores() const { return voices_.at(0).stores; }
+  const std::vector<int32_t>& publishedOuts() const { return pubOuts_; }
   bool readsBeatPhase() const { return phase_; }
   const AudioContext::InputSettings& settings() const { return settings_; }
   int numVoices() const { return numVoices_; }
@@ -2075,7 +2207,30 @@ class TracedSynth
     }
     std::fprintf(f, "], \"outs\": [");
     for (size_t i = 0; i < outs_.size(); ++i) std::fprintf(f, "%s%d", i ? ", " : "", outs_[i]);
-    std::fprintf(f, "]}\n");
+    std::fprintf(f, "]");
+    if (!published_.empty())  // a synth that publishes: its declarations, voice 0's store items, their graph outputs
+    {
+      std::fprintf(f, ", \"published\": [");
+      for (size_t s = 0; s < published_.size(); ++s)
+      {
+        const PublishDecl& d = published_[s];
+        std::fprintf(f, "%s{\"name\": \"%s\", \"max_frames\": %d, \"max_voices\": %d, \"channels\": %d, "
+                        "\"octaves_down\": %d}", s ? ", " : "", d.name.c_str(), d.maxFrames, d.maxVoices, d.channels,
+                     d.octavesDown);
+      }
+      std::fprintf(f, "], \"stores\": [");
+      const std::vector<PublishStore>& st = voices_[0].stores;
+      for (size_t k = 0; k < st.size(); ++k)
+      {
+        std::fprintf(f, "%s{\"signal\": %d, \"frames\": %d, \"rows\": [", k ? ", " : "", st[k].signal, st[k].frames);
+        for (size_t j = 0; j < st[k].rows.size(); ++j) std::fprintf(f, "%s%d", j ? ", " : "", st[k].rows[j]);
+        std::fprintf(f, "]}");
+      }
+      std::fprintf(f, "], \"published_outs\": [");
+      for (size_t i = 0; i < pubOuts_.size(); ++i) std::fprintf(f, "%s%d", i ? ", " : "", pubOuts_[i]);
+      std::fprintf(f, "]");
+    }
+    std::fprintf(f, "}\n");
   }
 
   // Create the banks for `instruments` instruments (needs a GPU): the router and Voice bank over
@@ -2085,7 +2240,7 @@ class TracedSynth
   {
     if (nodes_.empty()) throw Error(MLB_ERR_INVALID, "mlb::tr::TracedSynth: trace() first");
     if (instruments < 1) throw Error(MLB_ERR_INVALID, "mlb::tr::TracedSynth: instruments must be positive");
-    bank_.reset(), buses_.reset(), times_.reset(), ctrl_.reset(), voiceBank_.reset(), routers_.reset();
+    pubBank_.reset(), bank_.reset(), buses_.reset(), times_.reset(), ctrl_.reset(), voiceBank_.reset(), routers_.reset();
     const AudioContext::InputSettings& s = settings_;
     const int G = instruments, NR = lanesPerInstrument(), V = G * NR;
     instruments_ = G, lanesPer_ = NR;
@@ -2118,8 +2273,18 @@ class TracedSynth
       times_.reset(new ProcessTimeBank(G, sampleRate_));
       times_->setVoiceMap(inst.data(), V);
     }
-    bank_.reset(new DeviceBank(nodes_, outs_, V, flags));
+    std::vector<int32_t> outs = outs_;  // the audio outputs, then the published rows
+    outs.insert(outs.end(), pubOuts_.begin(), pubOuts_.end());
+    bank_.reset(new DeviceBank(nodes_, outs, V, flags));
     buses_.reset(new Buses(V, G, busFirst.data(), busCount.data()));
+    if (!published_.empty())
+    {
+      std::vector<mlb_published_signal> sig;
+      for (const PublishDecl& d : published_) sig.push_back({d.maxFrames, d.maxVoices, d.channels, d.octavesDown});
+      std::vector<mlb_published_store> st;
+      for (const PublishStore& k : voices_[0].stores) st.push_back({k.signal, k.frames});
+      pubBank_.reset(new PublishedBank(V, G, busFirst.data(), busCount.data(), sig, st));
+    }
     overflow_.assign((size_t)G, 0);
     for (size_t i = 0; i < nodes_.size(); ++i)
       for (int l = 0; l < V; ++l) loadWords(*bank_, (int)i, l, voices_[(size_t)laneVoice(l % NR)].nodes[i]);
@@ -2153,10 +2318,16 @@ class TracedSynth
                const mlb_transport* transports, int nTransports, float* bus, int nBlocks)
   {
     mlb_graph* graph = bank().handle();
-    check(mlb_synth_process_context_host(routers_->handle(), voiceBank_->handle(), ctrl_ ? ctrl_->handle() : nullptr,
-                                         times_ ? times_->handle() : nullptr, graph, buses_->handle(), offsets, events,
-                                         nEvents, times_ ? timeOffsets : nullptr, times_ ? transports : nullptr,
-                                         times_ ? nTransports : 0, nullptr, nullptr, bus, nBlocks));
+    if (pubBank_ && pubBank_->planes() > 0)  // K14 after the bus sum in every time chunk
+      check(mlb_synth_process_published_host(
+          routers_->handle(), voiceBank_->handle(), ctrl_ ? ctrl_->handle() : nullptr, times_ ? times_->handle() : nullptr,
+          graph, buses_->handle(), pubBank_->handle(), offsets, events, nEvents, times_ ? timeOffsets : nullptr,
+          times_ ? transports : nullptr, times_ ? nTransports : 0, bus, nBlocks));
+    else
+      check(mlb_synth_process_context_host(routers_->handle(), voiceBank_->handle(), ctrl_ ? ctrl_->handle() : nullptr,
+                                           times_ ? times_->handle() : nullptr, graph, buses_->handle(), offsets, events,
+                                           nEvents, times_ ? timeOffsets : nullptr, times_ ? transports : nullptr,
+                                           times_ ? nTransports : 0, nullptr, nullptr, bus, nBlocks));
     // A voice's record holds MLB_VOICE_MAX_EVENTS note events per vector (in unison every note event goes to every
     // voice); the router drops and counts the rest, where the reference's Voice would have written them all.
     std::vector<int64_t> overflow((size_t)instruments_);
@@ -2170,6 +2341,44 @@ class TracedSynth
                      " note events found their voice's record full (" + std::to_string(MLB_VOICE_MAX_EVENTS) +
                      " per voice and vector) and were dropped; this call's bus rows differ from the reference")
                         .c_str());
+  }
+
+  // getPublishedSignals()[name]->readLatest(dest, frames) of every instrument in one call (MLSignalProcessor.cpp:19-28):
+  // dest [instruments][frames * channels] (what a read does not fill is zero), counts [instruments] the floats read.
+  void readLatest(const Path& name, int frames, float* dest, int32_t* counts)
+  {
+    publishedBank().read(signalIndex(name), MLB_PUBLISHED_READ_LATEST, frames, dest, counts);
+  }
+  // ...->read(dest, frames): the oldest frames, consumed; counts the floats read
+  void read(const Path& name, int frames, float* dest, int32_t* counts)
+  {
+    publishedBank().read(signalIndex(name), MLB_PUBLISHED_READ, frames, dest, counts);
+  }
+  // ...->peekLatest(dest, frames): the newest frames, nothing consumed; counts 1 where they were copied, 0 where fewer
+  // were available (the reference copies nothing then, and dest stays zero here)
+  void peekLatest(const Path& name, int frames, float* dest, int32_t* counts)
+  {
+    publishedBank().read(signalIndex(name), MLB_PUBLISHED_PEEK, frames, dest, counts);
+  }
+  // ...->getAvailableFrames() into counts [instruments]
+  void availableFrames(const Path& name, int32_t* counts)
+  {
+    publishedBank().read(signalIndex(name), MLB_PUBLISHED_AVAILABLE, 0, nullptr, counts);
+  }
+
+ private:
+  PublishedBank& publishedBank() const
+  {
+    if (!pubBank_)
+      throw Error(MLB_ERR_INVALID, bank_ ? "mlb::tr::TracedSynth: the synth publishes no signal"
+                                         : "mlb::tr::TracedSynth: compile() first");
+    return *pubBank_;
+  }
+  int signalIndex(const Path& name) const
+  {
+    for (size_t s = 0; s < published_.size(); ++s)
+      if (published_[s].name == name) return (int)s;
+    throw Error(MLB_ERR_INVALID, ("mlb::tr::TracedSynth: no published signal named " + name).c_str());
   }
 };
 

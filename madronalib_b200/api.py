@@ -118,6 +118,13 @@ def lib() -> ctypes.CDLL:
     L.mlb_buses_destroy.argtypes = [_vp]
     L.mlb_buses_sum_device.argtypes = [_vp, _vp, _vp, ctypes.c_int, ctypes.c_int, _vp]
     L.mlb_synth_process_buses_host.argtypes = [_vp, _vp, _vp, _vp, _vp, ctypes.c_int]
+    L.mlb_published_create.argtypes = [ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, ctypes.c_int, _vp, ctypes.c_int, _vp]
+    L.mlb_published_destroy.argtypes = [_vp]
+    L.mlb_published_clear.argtypes = [_vp]
+    L.mlb_published_planes.argtypes = [_vp]
+    L.mlb_published_process_device.argtypes = [_vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
+    L.mlb_published_read_device.argtypes = [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp]
+    L.mlb_published_read_host.argtypes = [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _vp]
     L.mlb_synth_process_controllers_host.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int]
     L.mlb_routers_create.argtypes = [ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _vp, ctypes.c_int, _vp]
     L.mlb_routers_destroy.argtypes = [_vp]
@@ -654,6 +661,51 @@ class Buses(_Handle):
         one kernel launch, no allocation or synchronisation (capturable into a CUDA graph)."""
         _check(lib().mlb_buses_sum_device(self._h, _ptr(rows), _ptr(out), int(n_planes), int(n_blocks),
                                           stream or None))
+
+
+class PublishedBank(_Handle):
+    """Published signals of G instruments (mlb_published_*): per instrument and signal the ring of the reference's
+    SignalProcessor::PublishedSignal.  signals: (max_frames, max_voices, channels, octaves_down) per signal; stores:
+    (signal, frames) per storePublishedSignal call of processVoice, in call order, each owning `channels` consecutive
+    published planes.  Instrument g's voices are [first[g], first[g] + count[g]) of a V-voice bank."""
+
+    _destroy = "mlb_published_destroy"
+    READ_LATEST, READ, PEEK, AVAILABLE = 0, 1, 2, 3
+
+    def __init__(self, n_voices: int, first, count, signals, stores):
+        fv = np.ascontiguousarray(first, np.int32)
+        vc = np.ascontiguousarray(count, np.int32)
+        if fv.ndim != 1 or fv.shape != vc.shape:
+            raise ValueError(f"PublishedBank: `first` and `count` must be 1-D of one length, got {fv.shape} and {vc.shape}")
+        sig = np.ascontiguousarray(np.asarray(signals, np.int32).reshape(-1, 4))
+        st = np.ascontiguousarray(np.asarray(stores, np.int32).reshape(-1, 2))
+        self.n_voices, self.n_instruments = int(n_voices), int(fv.shape[0])
+        self.channels = [int(c) for c in sig[:, 2]]
+        h = ctypes.c_void_p()
+        _check(lib().mlb_published_create(self.n_voices, self.n_instruments, fv.ctypes.data, vc.ctypes.data,
+                                          sig.ctypes.data, len(sig), st.ctypes.data if len(st) else None, len(st),
+                                          ctypes.byref(h)))
+        self._h = h
+
+    @property
+    def planes(self) -> int:
+        return int(lib().mlb_published_planes(self._h))
+
+    def clear(self) -> None:
+        _check(lib().mlb_published_clear(self._h))
+
+    def process_device(self, rows, plane0: int, n_planes: int, n_blocks: int, stream: int = 0) -> None:
+        """rows [T][n_planes][V][64] (device), the published planes from plane0: one launch on ``stream``."""
+        _check(lib().mlb_published_process_device(self._h, _ptr(rows), int(plane0), int(n_planes), int(n_blocks),
+                                                  stream or None))
+
+    def read(self, signal: int, mode: int, frames: int = 0):
+        """One read of every instrument -> (dest [G][frames * channels] float32, counts [G] int32); see mlb200.h."""
+        dest = np.zeros((self.n_instruments, int(frames) * self.channels[signal]), np.float32)
+        counts = np.zeros(self.n_instruments, np.int32)
+        _check(lib().mlb_published_read_host(self._h, int(signal), int(mode), int(frames),
+                                             dest.ctypes.data if dest.size else None, counts.ctypes.data))
+        return dest, counts
 
 
 class _ListBank(_Handle):

@@ -19,11 +19,11 @@ constexpr int kBusAhead = 8;  // voice rows in flight per warp
 
 struct BusArgs
 {
-  const float* rows;     // [T][P][V][64]
+  const float* rows;     // [T][stride][V][64]: planes 0..P-1 of each block are summed
   float* bus;            // [T][P][G][64]
   const int32_t* first;  // [G]
   const int32_t* count;  // [G]
-  int V, G;
+  int V, G, P, stride;
   long long n_items;     // T * P * G
 };
 
@@ -41,8 +41,9 @@ __global__ void __launch_bounds__(32 * kBusWarps) bus_sum_kernel(BusArgs a)
   const int lane = threadIdx.x & 31;
   const int g = (int)(w % a.G);
   const long long tp = w / a.G;  // t * P + p
+  const long long row = tp + (tp / a.P) * (a.stride - a.P);  // t * stride + p
   const int first = __ldg(a.first + g), count = __ldg(a.count + g);
-  const float2* src = reinterpret_cast<const float2*>(a.rows + ((size_t)tp * a.V + first) * MLB_BLOCK) + lane;
+  const float2* src = reinterpret_cast<const float2*>(a.rows + ((size_t)row * a.V + first) * MLB_BLOCK) + lane;
   float2 acc = make_float2(0.f, 0.f);
   for (int i = 0; i < count; i += kBusAhead)
   {

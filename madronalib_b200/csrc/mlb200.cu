@@ -32,6 +32,7 @@
 #include "controller_kernel.cuh"
 #include "router_kernel.cuh"
 #include "process_time_kernel.cuh"
+#include "publish_kernel.cuh"
 #include "generic_kernel.cuh"
 
 using namespace mlb;
@@ -2595,6 +2596,7 @@ struct SynthCall
   const mlb_transport* transports = nullptr;
   int n_transports = 0;
   mlb_buses* b = nullptr;
+  mlb_published* p = nullptr;  // with b: K14 after the bus sum, over the graph's last mlb_published_planes outputs
   float *out = nullptr, *mix = nullptr, *bus = nullptr;
   int run() const;  // the driver
 };
@@ -2651,15 +2653,13 @@ extern "C" int mlb_buses_create(int n_voices, int n_buses, const int32_t* first_
   return MLB_OK;
 }
 
-extern "C" int mlb_buses_sum_device(mlb_buses* b, const float* rows_dev, float* bus_dev, int n_planes, int n_blocks,
-                                    void* stream)
+// rows [T][stride][V][64]: planes 0..n_planes-1 of every block are summed into bus [T][n_planes][G][64]
+static int bus_sum(mlb_buses* b, const float* rows_dev, float* bus_dev, int n_planes, int stride, int n_blocks,
+                   void* stream)
 {
-  if (!b || !rows_dev || !bus_dev) return fail(MLB_ERR_INVALID, "null argument");
-  if (n_planes <= 0) return fail(MLB_ERR_INVALID, "n_planes must be positive (got %d)", n_planes);
-  if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive (got %d)", n_blocks);
   BusArgs a;
   a.rows = rows_dev, a.bus = bus_dev, a.first = b->d_table.get(), a.count = b->d_table.get() + b->G;
-  a.V = b->V, a.G = b->G;
+  a.V = b->V, a.G = b->G, a.P = n_planes, a.stride = stride;
   a.n_items = (long long)n_blocks * n_planes * b->G;
   const long long grid = (a.n_items + kBusWarps - 1) / kBusWarps;
   if (grid > 0x7FFFFFFFLL) return fail(MLB_ERR_INVALID, "%lld bus rows exceed one launch", a.n_items);
@@ -2667,6 +2667,15 @@ extern "C" int mlb_buses_sum_device(mlb_buses* b, const float* rows_dev, float* 
   ++g_launches;
   CU_CHECK(cudaGetLastError());
   return MLB_OK;
+}
+
+extern "C" int mlb_buses_sum_device(mlb_buses* b, const float* rows_dev, float* bus_dev, int n_planes, int n_blocks,
+                                    void* stream)
+{
+  if (!b || !rows_dev || !bus_dev) return fail(MLB_ERR_INVALID, "null argument");
+  if (n_planes <= 0) return fail(MLB_ERR_INVALID, "n_planes must be positive (got %d)", n_planes);
+  if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive (got %d)", n_blocks);
+  return bus_sum(b, rows_dev, bus_dev, n_planes, n_planes, n_blocks, stream);
 }
 
 // Contract E with per-instrument output: the graph's rows of a chunk go to a device scratch of one chunk (g->d_out),
@@ -3287,8 +3296,196 @@ extern "C" int mlb_routers_process_host(mlb_routers* r, const int32_t* offsets_h
 }
 
 // The checks of contract E from raw events (the routed and context entry points), then the driver.
+// ------------------------------------------------------------------------------------------
+// Published signals (K14, publish_kernel.cuh)
+
+struct mlb_published
+{
+  // declared first, so released last: the buffers below are freed first, and cudaFree waits for the device
+  LiveCount live;
+  Stream stream;  // the host reads
+  int V = 0, G = 0, Q = 0;  // Q: published planes, the sum of the stores' channels
+  std::vector<mlb_published_signal> signals;
+  PubArgs args{};           // everything but rows, T, stride, plane0
+  DevBuf<int32_t> d_table;  // [2][G]: first voice, voice count
+  DevBuf<float> d_ring;
+  DevBuf<uint32_t> d_state;  // [n_signals][G][3]
+  DevBuf<float> d_dest;      // staging of mlb_published_read_host
+  DevBuf<int32_t> d_counts;
+};
+
+extern "C" int mlb_published_destroy(mlb_published* p)
+{
+  delete p;
+  return MLB_OK;
+}
+
+extern "C" int mlb_published_clear(mlb_published* p)
+{
+  if (!p) return fail(MLB_ERR_INVALID, "null published bank");
+  CU_CHECK(cudaMemset(p->d_state.get(), 0, p->d_state.bytes()));
+  CU_CHECK(cudaMemset(p->d_ring.get(), 0, p->d_ring.bytes()));
+  return MLB_OK;
+}
+
+extern "C" int mlb_published_planes(const mlb_published* p) { return p ? p->Q : 0; }
+
+extern "C" int mlb_published_create(int n_voices, int n_instruments, const int32_t* first_voice,
+                                    const int32_t* voice_count, const mlb_published_signal* signals, int n_signals,
+                                    const mlb_published_store* stores, int n_stores, mlb_published** out)
+{
+  if (!out) return fail(MLB_ERR_INVALID, "out is null");
+  *out = nullptr;
+  if (n_voices <= 0) return fail(MLB_ERR_INVALID, "n_voices must be positive (got %d)", n_voices);
+  if (n_instruments < 1) return fail(MLB_ERR_INVALID, "n_instruments must be positive (got %d)", n_instruments);
+  if (!first_voice || !voice_count) return fail(MLB_ERR_INVALID, "null layout table");
+  if (n_signals < 1 || n_signals > MLB_PUBLISHED_MAX_SIGNALS || !signals)
+    return fail(MLB_ERR_INVALID, "%d signals: 1..%d are supported", n_signals, MLB_PUBLISHED_MAX_SIGNALS);
+  if (n_stores < 0 || n_stores > MLB_PUBLISHED_MAX_STORES || (n_stores > 0 && !stores))
+    return fail(MLB_ERR_INVALID, "%d stores: 0..%d are supported", n_stores, MLB_PUBLISHED_MAX_STORES);
+  for (int g = 0; g < n_instruments; ++g)
+    if (first_voice[g] < 0 || voice_count[g] < 0 || (int64_t)first_voice[g] + voice_count[g] > n_voices)
+      return fail(MLB_ERR_INVALID, "instrument %d: first voice %d, count %d is not a range of the %d voices", g,
+                  first_voice[g], voice_count[g], n_voices);
+  std::unique_ptr<mlb_published> p(new mlb_published);
+  PubArgs& a = p->args;
+  long long ring = 0;
+  for (int s = 0; s < n_signals; ++s)
+  {
+    const mlb_published_signal& d = signals[s];
+    if (d.max_frames < 1 || d.max_voices < 1 || d.channels < 1 || d.channels > MLB_BLOCK || d.octaves_down < 0 ||
+        d.octaves_down > 30)
+      return fail(MLB_ERR_INVALID, "signal %d: max_frames %d, max_voices %d, channels %d, octaves_down %d (want >= 1, "
+                  ">= 1, 1..64, 0..30)", s, d.max_frames, d.max_voices, d.channels, d.octaves_down);
+    const long long want = (long long)d.max_frames * d.channels * d.max_voices;
+    long long size = MLB_BLOCK;  // DSPBuffer::resize, MLDSPBuffer.h:104-130
+    while (size < want) size <<= 1;
+    if (size > (1ll << 28)) return fail(MLB_ERR_INVALID, "signal %d: a ring of %lld floats is too large", s, size);
+    PubSignal& sg = a.sig[s];
+    sg.channels = d.channels, sg.octaves = d.octaves_down, sg.size = (int)size;
+    sg.first_item = 0, sg.n_items = 0, sg.frames = 0, sg.ring = ring;
+    ring += size * n_instruments;
+  }
+  // the items of each signal, contiguous and in call order; planes in store order
+  int plane = 0, n_items = 0;
+  for (int k = 0; k < n_stores; ++k)
+  {
+    const mlb_published_store& st = stores[k];
+    if (st.signal < 0 || st.signal >= n_signals)
+      return fail(MLB_ERR_INVALID, "store %d: signal %d is not one of the %d signals", k, st.signal, n_signals);
+    if (st.frames < 0 || st.frames > MLB_BLOCK || st.frames > signals[st.signal].max_frames)
+      return fail(MLB_ERR_INVALID, "store %d: %d frames is not in 0..min(64, max_frames %d) of signal %d", k, st.frames,
+                  signals[st.signal].max_frames, st.signal);
+    plane += signals[st.signal].channels;
+  }
+  for (int s = 0; s < n_signals; ++s)
+  {
+    a.sig[s].first_item = n_items;
+    int q = 0;
+    for (int k = 0; k < n_stores; ++k)
+    {
+      if (stores[k].signal == s)
+      {
+        a.item[n_items].frames = stores[k].frames, a.item[n_items].plane = q;
+        a.sig[s].frames += stores[k].frames;
+        ++a.sig[s].n_items, ++n_items;
+      }
+      q += signals[stores[k].signal].channels;
+    }
+  }
+  MLB_TRY(ensure_init());
+  p->live.arm();
+  p->V = n_voices, p->G = n_instruments, p->Q = plane;
+  p->signals.assign(signals, signals + n_signals);
+  a.V = n_voices, a.G = n_instruments, a.n_signals = n_signals;
+  const size_t bytes = (size_t)n_instruments * sizeof(int32_t);
+  MLB_TRY(p->d_table.alloc(2 * bytes, "published bank layout"));
+  MLB_TRY(p->d_ring.alloc((size_t)ring * 4, "published rings"));
+  MLB_TRY(p->d_state.alloc((size_t)n_signals * n_instruments * 3 * 4, "published ring indices"));
+  MLB_TRY(p->stream.create(cudaStreamNonBlocking));
+  CU_CHECK(cudaMemcpy(p->d_table.get(), first_voice, bytes, cudaMemcpyHostToDevice));
+  CU_CHECK(cudaMemcpy(p->d_table.get() + n_instruments, voice_count, bytes, cudaMemcpyHostToDevice));
+  a.first = p->d_table.get(), a.count = p->d_table.get() + n_instruments;
+  a.ring = p->d_ring.get(), a.state = p->d_state.get();
+  MLB_TRY(mlb_published_clear(p.get()));
+  *out = p.release();
+  return MLB_OK;
+}
+
+extern "C" int mlb_published_process_device(mlb_published* p, const float* rows_dev, int plane0, int n_planes,
+                                            int n_blocks, void* stream)
+{
+  if (!p || !rows_dev) return fail(MLB_ERR_INVALID, "null argument");
+  if (n_blocks <= 0) return fail(MLB_ERR_INVALID, "n_blocks must be positive (got %d)", n_blocks);
+  if (plane0 < 0 || plane0 + p->Q > n_planes)
+    return fail(MLB_ERR_INVALID, "published planes %d..%d are not within the %d planes", plane0, plane0 + p->Q - 1,
+                n_planes);
+  if (p->Q == 0) return MLB_OK;
+  PubArgs a = p->args;
+  a.rows = rows_dev, a.T = n_blocks, a.stride = n_planes, a.plane0 = plane0;
+  const int items = a.n_signals * a.G;
+  publish_kernel<<<(unsigned)((items + kPubWarps - 1) / kPubWarps), 32 * kPubWarps, 0, (cudaStream_t)stream>>>(a);
+  ++g_launches;
+  CU_CHECK(cudaGetLastError());
+  return MLB_OK;
+}
+
+static int published_read_check(const mlb_published* p, int signal, int mode, int frames, const void* dest)
+{
+  if (!p) return fail(MLB_ERR_INVALID, "null published bank");
+  if (signal < 0 || signal >= (int)p->signals.size())
+    return fail(MLB_ERR_INVALID, "signal %d is not one of the %d signals", signal, (int)p->signals.size());
+  if (mode < MLB_PUBLISHED_READ_LATEST || mode > MLB_PUBLISHED_AVAILABLE)
+    return fail(MLB_ERR_INVALID, "read mode %d is not an MLB_PUBLISHED_* mode", mode);
+  if (mode != MLB_PUBLISHED_AVAILABLE && (frames < 0 || (frames > 0 && !dest)))
+    return fail(MLB_ERR_INVALID, "a read of %d frames into %p", frames, dest);
+  if ((long long)frames * p->signals[(size_t)signal].channels > (1ll << 28))
+    return fail(MLB_ERR_INVALID, "a read of %d frames is too large", frames);
+  return MLB_OK;
+}
+
+static int published_read(mlb_published* p, int signal, int mode, int frames, float* dest_dev, int32_t* counts_dev,
+                          cudaStream_t stream)
+{
+  PubReadArgs a;
+  const PubSignal& sg = p->args.sig[signal];
+  a.ring = p->d_ring.get() + sg.ring, a.state = p->d_state.get() + (size_t)signal * p->G * 3;
+  a.dest = mode == MLB_PUBLISHED_AVAILABLE ? nullptr : dest_dev, a.counts = counts_dev;
+  a.G = p->G, a.size = sg.size, a.channels = sg.channels, a.mode = mode, a.frames = mode == MLB_PUBLISHED_AVAILABLE ? 0 : frames;
+  publish_read_kernel<<<(unsigned)((p->G + kPubWarps - 1) / kPubWarps), 32 * kPubWarps, 0, stream>>>(a);
+  ++g_launches;
+  CU_CHECK(cudaGetLastError());
+  return MLB_OK;
+}
+
+extern "C" int mlb_published_read_device(mlb_published* p, int signal, int mode, int frames, float* dest_dev,
+                                         int32_t* counts_dev, void* stream)
+{
+  MLB_TRY(published_read_check(p, signal, mode, frames, dest_dev));
+  return published_read(p, signal, mode, frames, dest_dev, counts_dev, (cudaStream_t)stream);
+}
+
+extern "C" int mlb_published_read_host(mlb_published* p, int signal, int mode, int frames, float* dest_host,
+                                       int32_t* counts_host)
+{
+  MLB_TRY(published_read_check(p, signal, mode, frames, dest_host));
+  const size_t floats = mode == MLB_PUBLISHED_AVAILABLE ? 0 : (size_t)frames * p->signals[(size_t)signal].channels * p->G;
+  MLB_TRY(p->d_dest.ensure(std::max<size_t>(floats, 1) * 4, "staging"));
+  MLB_TRY(p->d_counts.ensure((size_t)p->G * 4, "staging"));
+  cudaStream_t s = p->stream.get();
+  const int rc = [&]() -> int
+  {
+    MLB_TRY(published_read(p, signal, mode, frames, p->d_dest.get(), p->d_counts.get(), s));
+    if (floats && dest_host)
+      CU_CHECK(cudaMemcpyAsync(dest_host, p->d_dest.get(), floats * 4, cudaMemcpyDeviceToHost, s));
+    if (counts_host) CU_CHECK(cudaMemcpyAsync(counts_host, p->d_counts.get(), (size_t)p->G * 4, cudaMemcpyDeviceToHost, s));
+    return MLB_OK;
+  }();
+  return drain(rc, {s});
+}
+
 static int synth_routed(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb, mlb_process_time* pt, mlb_graph* g,
-                        mlb_buses* b, const int32_t* offsets_host, const mlb_event* events_host, int n_events,
+                        mlb_buses* b, mlb_published* p, const int32_t* offsets_host, const mlb_event* events_host, int n_events,
                         const int32_t* time_offsets_host, const mlb_transport* transports_host, int n_transports,
                         float* out_host, float* mix_host, float* bus_host, int n_blocks)
 {
@@ -3312,6 +3509,10 @@ static int synth_routed(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb, mlb
     return fail(MLB_ERR_INVALID, "controller bank's voice map has %d voices, graph has %d (mlb_controllers_set_voice_map)",
                 cb->V, g->V);
   if (b && b->V != g->V) return fail(MLB_ERR_INVALID, "buses are laid over %d voices, graph has %d", b->V, g->V);
+  if (p && !b) return fail(MLB_ERR_INVALID, "a published bank needs buses");
+  if (p && p->V != g->V) return fail(MLB_ERR_INVALID, "published bank is laid over %d voices, graph has %d", p->V, g->V);
+  if (p && (int)g->outs.size() <= p->Q)
+    return fail(MLB_ERR_INVALID, "graph has %d outputs: none besides the %d published planes", (int)g->outs.size(), p->Q);
   if (pt && pt->G != r->G)
     return fail(MLB_ERR_INVALID, "router bank has %d instruments, process-time bank %d", r->G, pt->G);
   if (pt && pt->V != g->V)
@@ -3327,6 +3528,7 @@ static int synth_routed(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb, mlb
   c.vb = vb, c.g = g, c.n_blocks = n_blocks, c.out = out_host, c.mix = mix_host, c.b = b, c.bus = bus_host;
   c.r = r, c.offsets = offsets_host, c.events = events_host, c.n_events = n_events, c.n_changes = n_changes, c.cb = cb;
   c.pt = pt, c.time_offsets = time_offsets_host, c.transports = transports_host, c.n_transports = n_transports;
+  c.p = p && p->Q ? p : nullptr;
   return c.run();
 }
 
@@ -3341,11 +3543,12 @@ static int synth_routed(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb, mlb
 int SynthCall::run() const
 {
   MLB_TRY(ensure_init());
-  const size_t V = (size_t)g->V, T = (size_t)n_blocks, n_out = g->outs.size();
+  const size_t V = (size_t)g->V, T = (size_t)n_blocks, n_rows = g->outs.size();
+  const size_t n_out = n_rows - (p ? (size_t)p->Q : 0);  // the audio planes; the published planes follow them
   const size_t G1 = (size_t)(r ? r->G : cb ? cb->G : 0) + 1;  // pt->G is r->G
   const int Tc = synth_chunk_blocks(g, n_blocks, n_planes);
   if (out) MLB_TRY(g->d_out.ensure(T * n_out * V * MLB_BLOCK * 4, "staging"));
-  if (b) MLB_TRY(g->d_out.ensure((size_t)Tc * n_out * V * MLB_BLOCK * 4, "staging"));
+  if (b) MLB_TRY(g->d_out.ensure((size_t)Tc * n_rows * V * MLB_BLOCK * 4, "staging"));
   if (b) MLB_TRY(b->d_out.ensure(T * n_out * b->G * MLB_BLOCK * 4, "staging"));
   if (mix) MLB_TRY(g->d_mix.ensure(T * n_out * MLB_BLOCK * 4, "staging"));
   if (r)
@@ -3401,7 +3604,8 @@ int SynthCall::run() const
           if (b)
           {
             MLB_TRY(graph_process(g, vb->d_out.get(), n_planes, g->d_out.get(), nullptr, t1 - t0, s));
-            return mlb_buses_sum_device(b, g->d_out.get(), b->d_out.get() + t0 * bus_floats, (int)n_out, t1 - t0, s);
+            MLB_TRY(bus_sum(b, g->d_out.get(), b->d_out.get() + t0 * bus_floats, (int)n_out, (int)n_rows, t1 - t0, s));
+            return p ? mlb_published_process_device(p, g->d_out.get(), (int)n_out, (int)n_rows, t1 - t0, s) : MLB_OK;
           }
           return graph_process(g, vb->d_out.get(), n_planes, out ? g->d_out.get() + t0 * row_floats : nullptr,
                                mix ? g->d_mix.get() + t0 * n_out * MLB_BLOCK : nullptr, t1 - t0, s);
@@ -3424,7 +3628,7 @@ extern "C" int mlb_synth_process_routed_host(mlb_routers* r, mlb_voices* vb, mlb
                                              int n_events, float* out_host, float* mix_host, float* bus_host,
                                              int n_blocks)
 {
-  return synth_routed(r, vb, cb, nullptr, g, b, offsets_host, events_host, n_events, nullptr, nullptr, 0, out_host,
+  return synth_routed(r, vb, cb, nullptr, g, b, nullptr, offsets_host, events_host, n_events, nullptr, nullptr, 0, out_host,
                       mix_host, bus_host, n_blocks);
 }
 
@@ -3435,8 +3639,19 @@ extern "C" int mlb_synth_process_context_host(mlb_routers* r, mlb_voices* vb, ml
                                               int n_transports, float* out_host, float* mix_host, float* bus_host,
                                               int n_blocks)
 {
-  return synth_routed(r, vb, cb, pt, g, b, offsets_host, events_host, n_events, time_offsets_host, transports_host,
-                      n_transports, out_host, mix_host, bus_host, n_blocks);
+  return synth_routed(r, vb, cb, pt, g, b, nullptr, offsets_host, events_host, n_events, time_offsets_host,
+                      transports_host, n_transports, out_host, mix_host, bus_host, n_blocks);
+}
+
+extern "C" int mlb_synth_process_published_host(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb,
+                                                mlb_process_time* pt, mlb_graph* g, mlb_buses* b, mlb_published* p,
+                                                const int32_t* offsets_host, const mlb_event* events_host, int n_events,
+                                                const int32_t* time_offsets_host, const mlb_transport* transports_host,
+                                                int n_transports, float* bus_host, int n_blocks)
+{
+  if (!p) return fail(MLB_ERR_INVALID, "null published bank");
+  return synth_routed(r, vb, cb, pt, g, b, p, offsets_host, events_host, n_events, time_offsets_host, transports_host,
+                      n_transports, nullptr, nullptr, bus_host, n_blocks);
 }
 
 // ------------------------------------------------------------------------------------------
