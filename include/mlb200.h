@@ -860,6 +860,27 @@ int mlb_synth_process_published_host(mlb_routers* r, mlb_voices* vb, mlb_control
                                      const mlb_transport* transports_host, int n_transports, float* bus_host,
                                      int n_blocks);
 
+/* ---- Restart: lane-selective resets (DESIGN.md "Restart") ----
+ * Each sets the listed voices (graph, Voice bank) or instruments (the other banks) to the state a freshly
+ * constructed object holds, and leaves every other one untouched, bit for bit:
+ *   graph        state words from the last mlb_graph_set_state (or creation), the voice's delay rings and rows zero;
+ *                coefficients and the global delay write index are kept
+ *   Voice bank   state words as mlb_voices_create wrote them, LinearGlide rows zero; coefficients kept
+ *   routers      as mlb_routers_clear leaves an instrument: its overflow and unsupported counters are kept
+ *   controllers  as mlb_controllers_clear leaves an instrument
+ *   process time the words mlb_process_time_create wrote (not ProcessTime::clear, which keeps omega_)
+ *   published    rings empty, indices and decimation counter 0, for every signal
+ * The list may repeat an index (it acts once).  MLB_ERR_INVALID, naming the index, when an index is out of range,
+ * the list is NULL with n > 0 or n < 0: then nothing is written.  n = 0 launches nothing.  Otherwise one launch on the
+ * bank's stream, finished when the call returns (as the *_clear calls): any later call sees it.  The reset must not
+ * overlap a *_device call of the same bank still running on another stream. */
+int mlb_graph_reset_voices(mlb_graph* g, const int32_t* voices, int n);
+int mlb_voices_reset(mlb_voices* vb, const int32_t* voices, int n);
+int mlb_routers_reset(mlb_routers* r, const int32_t* instruments, int n);
+int mlb_controllers_reset(mlb_controllers* cb, const int32_t* instruments, int n);
+int mlb_process_time_reset(mlb_process_time* pt, const int32_t* instruments, int n);
+int mlb_published_reset(mlb_published* p, const int32_t* instruments, int n);
+
 #ifdef __cplusplus
 }
 #endif

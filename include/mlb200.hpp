@@ -636,6 +636,9 @@ class DeviceBank
   }
   uint32_t stateWord(int node, int slot, int row) const { return state_[(size_t)(st_off_[node] + slot) * rows_ + row]; }
   void clear() { check(mlb_graph_clear_delays(g_)); }
+  // the listed rows to the state of the last commit() and empty delay memory, as freshly built objects
+  // (mlb_graph_reset_voices); coefficients kept
+  void reset(const std::vector<int32_t>& rows) { check(mlb_graph_reset_voices(g_, rows.data(), (int)rows.size())); }
 
   // n_blocks successive Bank::operator() calls: in [T][n_in][rows][64], out [T][n_out][rows][64]
   void process(const float* in, float* out, float* mix, int n_blocks) { check(mlb_graph_process_host(g_, in, out, mix, n_blocks)); }
@@ -670,6 +673,8 @@ class VoiceBank
   int voices() const { return n_; }
   mlb_voices* handle() const { return vb_; }
   void setMainVoices(const int32_t* mainVoice) { check(mlb_voices_set_main_voices(vb_, mainVoice)); }
+  // the listed voices as the constructor left them (mlb_voices_reset)
+  void reset(const std::vector<int32_t>& voices) { check(mlb_voices_reset(vb_, voices.data(), (int)voices.size())); }
   // events [nBlocks][voices]; out [nBlocks][MLB_VOICE_ROWS][voices][64]
   void process(const mlb_voice_events* events, float* out, int nBlocks, unsigned rowMask = 0xFFu)
   {
@@ -738,6 +743,11 @@ class PublishedBank
   int planes() const { return mlb_published_planes(p_); }
   int channels(int signal) const { return signals_.at((size_t)signal).channels; }
   void clear() { check(mlb_published_clear(p_)); }
+  // the listed instruments' rings empty (mlb_published_reset)
+  void reset(const std::vector<int32_t>& instruments)
+  {
+    check(mlb_published_reset(p_, instruments.data(), (int)instruments.size()));
+  }
   // one read of `signal` for every instrument (mode MLB_PUBLISHED_*): dest [instruments][frames * channels], counts
   // [instruments]; host buffers
   void read(int signal, int mode, int frames, float* dest, int32_t* counts)
@@ -779,6 +789,11 @@ class ControllerBank
   int controllers() const { return controllers_; }
   mlb_controllers* handle() const { return c_; }
   void clear() { check(mlb_controllers_clear(c_)); }
+  // clear() of the listed instruments only (mlb_controllers_reset)
+  void reset(const std::vector<int32_t>& instruments)
+  {
+    check(mlb_controllers_reset(c_, instruments.data(), (int)instruments.size()));
+  }
   // voiceInstrument[nVoices]: each voice's instrument or -1; nullptr goes back to instrument rows
   void setVoiceMap(const int32_t* voiceInstrument, int nVoices) { check(mlb_controllers_set_voice_map(c_, voiceInstrument, nVoices)); }
   // device buffers, asynchronous on `stream`: offsets [nBlocks][instruments + 1] into changes ->
@@ -823,6 +838,11 @@ class RouterBank
   int voices() const { return voices_; }
   mlb_routers* handle() const { return r_; }
   void clear() { check(mlb_routers_clear(r_)); }
+  // clear() of the listed instruments only, counters kept (mlb_routers_reset)
+  void reset(const std::vector<int32_t>& instruments)
+  {
+    check(mlb_routers_reset(r_, instruments.data(), (int)instruments.size()));
+  }
   // per instrument, since creation; either pointer may be nullptr
   void counters(int64_t* overflow, int64_t* unsupported) { check(mlb_routers_counters(r_, overflow, unsupported)); }
   // host buffers: offsets [nBlocks][instruments + 1] into events -> records [nBlocks][voices], changeOffsets
@@ -876,6 +896,11 @@ class ProcessTimeBank
   mlb_process_time* handle() const { return p_; }
   // ProcessTime::clear() of every clock (dpdt_, active1_, playing1_ only, as in the reference)
   void clear() { check(mlb_process_time_clear(p_)); }
+  // the listed clocks as the constructor left them, omega_ included (mlb_process_time_reset)
+  void reset(const std::vector<int32_t>& instruments)
+  {
+    check(mlb_process_time_reset(p_, instruments.data(), (int)instruments.size()));
+  }
   // words [MLB_PT_WORDS][instruments]
   void getState(uint64_t* words) { check(mlb_process_time_get_state(p_, words)); }
   void setState(const uint64_t* words) { check(mlb_process_time_set_state(p_, words)); }

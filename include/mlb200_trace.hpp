@@ -1822,6 +1822,12 @@ class TracedProcessor
   void setCoef(int node, int word, int instance, float value) { bank().setCoef(node, word, instance, value); }
   void setStateWord(int node, int word, int instance, uint32_t value) { bank().setStateWord(node, word, instance, value); }
 
+  // Restart the listed instances between two calls: from the next vector each runs as a newly constructed copy of the
+  // process function (its state words as the last commit() uploaded them, its delay memory empty, its parameters
+  // kept); the others are untouched.  One launch, none for an empty list.  Frames the process() streaming shim has
+  // already computed and buffered are not recalled: they come out of the next process() call as before.
+  void restart(const std::vector<int>& instances) { bank().reset(std::vector<int32_t>(instances.begin(), instances.end())); }
+
   // n_blocks successive process calls for every instance in ONE kernel launch.
   // in [T][inputs][instances][64], out [T][outputs][instances][64], mix [T][outputs][64] (sum over instances).
   void processBlocks(const float* in, float* out, float* mix, int nBlocks) { bank().process(in, out, mix, nBlocks); }
@@ -2341,6 +2347,27 @@ class TracedSynth
                      " note events found their voice's record full (" + std::to_string(MLB_VOICE_MAX_EVENTS) +
                      " per voice and vector) and were dropped; this call's bus rows differ from the reference")
                         .c_str());
+  }
+
+  // Restart the listed instruments between two process() calls: from the next vector each behaves as a newly
+  // constructed AudioContext + Synth set up as at trace time (the reference's `ctxs[g] = make_unique<AudioContext>(..);
+  // synths[g] = make_unique<...>(..)`), fed only the events and transport updates from then on; the others are
+  // untouched, bit for bit.  The graph lanes go back to the words of the last commit(), so setParam values stay.  One
+  // launch per bank that holds state (routers, Voice rows, controllers and beat phase if built, graph, published
+  // signals if built), none for an empty list; an instrument out of range throws before anything is written.
+  void restart(const std::vector<int>& instruments)
+  {
+    DeviceBank& bank = this->bank();
+    const std::vector<int32_t> inst(instruments.begin(), instruments.end());
+    std::vector<int32_t> lanes;
+    for (int g : instruments)
+      for (int j = 0; j < lanesPer_; ++j) lanes.push_back(g * lanesPer_ + j);
+    routers_->reset(inst);  // first: it refuses an instrument out of range before any bank is written
+    voiceBank_->reset(lanes);
+    if (ctrl_) ctrl_->reset(inst);
+    if (times_) times_->reset(inst);
+    bank.reset(lanes);
+    if (pubBank_) pubBank_->reset(inst);
   }
 
   // getPublishedSignals()[name]->readLatest(dest, frames) of every instrument in one call (MLSignalProcessor.cpp:19-28):

@@ -157,6 +157,9 @@ def lib() -> ctypes.CDLL:
     L.mlb_mixbus_set_async.argtypes = [_vp, ctypes.c_int]
     L.mlb_graph_mix_wait.argtypes = [_vp, _vp]
     L.mlb_graph_set_mix_async.argtypes = [_vp, ctypes.c_int]
+    for fn in ("mlb_graph_reset_voices", "mlb_voices_reset", "mlb_routers_reset", "mlb_controllers_reset",
+               "mlb_process_time_reset", "mlb_published_reset"):
+        getattr(L, fn).argtypes = [_vp, _vp, ctypes.c_int]
     L.mlb_map_device.argtypes = [ctypes.c_int, _vp, _vp, _vp, _vp, ctypes.c_size_t, _vp]
     L.mlb_map_host.argtypes = [ctypes.c_int, _vp, _vp, _vp, _vp, ctypes.c_size_t]
     L.mlb_map_host_allocations.restype = ctypes.c_longlong
@@ -220,6 +223,13 @@ def _out_array(name: str, key: str, a, shape, new=np.empty) -> np.ndarray:
     if not (isinstance(a, np.ndarray) and a.dtype == np.float32 and a.flags["C_CONTIGUOUS"] and a.shape == shape):
         raise ValueError(f"{name}: `{key}` must be a C-contiguous float32 array of shape {shape}")
     return a
+
+
+def _reset(fn: str, h, indexes) -> None:
+    """The library's reset `fn` (mlb_graph_reset_voices, mlb_voices_reset, ...) of the voices or instruments in
+    `indexes`: synchronous, one kernel launch, none for an empty list."""
+    ix = np.ascontiguousarray(indexes, np.int32).reshape(-1)
+    _check(getattr(lib(), fn)(h, ix.ctypes.data if ix.size else None, int(ix.size)))
 
 
 def device_count() -> int:
@@ -405,6 +415,11 @@ class VoiceGraph(_Handle):
 
     def clear_delays(self) -> None:
         _check(lib().mlb_graph_clear_delays(self._h))
+
+    def reset_voices(self, voices) -> None:
+        """The listed voices as freshly created ones: state words of the last set_state, delay memory empty;
+        coefficients kept, the other voices untouched (mlb_graph_reset_voices)."""
+        _reset("mlb_graph_reset_voices", self._h, voices)
 
     def process_host(self, inp: Optional[np.ndarray], n_blocks: int, want_out: bool = True,
                      want_mix: bool = False, out: Optional[np.ndarray] = None,
@@ -625,6 +640,10 @@ class VoiceBank(_Handle):
         assert mv.shape == (self.n_voices,)
         _check(lib().mlb_voices_set_main_voices(self._h, mv.ctypes.data))
 
+    def reset(self, voices) -> None:
+        """The listed voices as the constructor left them (mlb_voices_reset)."""
+        _reset("mlb_voices_reset", self._h, voices)
+
     def process_host(self, events: np.ndarray, row_mask: int = 0xFF) -> np.ndarray:
         """events: [T][V] array of workloads.VOICE_EVENTS_DTYPE; returns out [T][8][V][64] f32
         (planes whose bit is clear in row_mask are left zero)."""
@@ -693,6 +712,10 @@ class PublishedBank(_Handle):
 
     def clear(self) -> None:
         _check(lib().mlb_published_clear(self._h))
+
+    def reset(self, instruments) -> None:
+        """clear() of the listed instruments only (mlb_published_reset)."""
+        _reset("mlb_published_reset", self._h, instruments)
 
     def process_device(self, rows, plane0: int, n_planes: int, n_blocks: int, stream: int = 0) -> None:
         """rows [T][n_planes][V][64] (device), the published planes from plane0: one launch on ``stream``."""
@@ -765,6 +788,10 @@ class ControllerBank(_ListBank):
     def clear(self) -> None:
         _check(lib().mlb_controllers_clear(self._h))
 
+    def reset(self, instruments) -> None:
+        """clear() of the listed instruments only (mlb_controllers_reset)."""
+        _reset("mlb_controllers_reset", self._h, instruments)
+
     def get_state(self):
         """(words [4][C][G] uint32, rows [C][G][64] f32); an idle glide's row is its target."""
         C, G = self.n_controllers, self.n_instruments
@@ -825,6 +852,10 @@ class ProcessTimeBank(_ListBank):
     def clear(self) -> None:
         """ProcessTime::clear() of every clock: dpdt_, active1_ and playing1_ only."""
         _check(lib().mlb_process_time_clear(self._h))
+
+    def reset(self, instruments) -> None:
+        """The listed clocks as the constructor left them, omega_ included (mlb_process_time_reset)."""
+        _reset("mlb_process_time_reset", self._h, instruments)
 
     def get_state(self) -> np.ndarray:
         """words [10][G] uint64: a float's bits in the low 32 bits, a double's bits, a bool as 0 / 1, a counter."""
@@ -1012,6 +1043,10 @@ class RouterBank(_Handle):
 
     def clear(self) -> None:
         _check(lib().mlb_routers_clear(self._h))
+
+    def reset(self, instruments) -> None:
+        """clear() of the listed instruments only, their overflow and unsupported counters kept (mlb_routers_reset)."""
+        _reset("mlb_routers_reset", self._h, instruments)
 
     def counters(self):
         """(overflow [G], unsupported [G]) int64, since creation."""

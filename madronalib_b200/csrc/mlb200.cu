@@ -33,6 +33,7 @@
 #include "router_kernel.cuh"
 #include "process_time_kernel.cuh"
 #include "publish_kernel.cuh"
+#include "restart_kernel.cuh"
 #include "generic_kernel.cuh"
 
 using namespace mlb;
@@ -790,6 +791,7 @@ struct mlb_graph
 
   // device SoA
   DevBuf<uint32_t> d_state;
+  DevBuf<uint32_t> d_state0;  // the words of the last mlb_graph_set_state (or of creation): a lane's start state
   DevBuf<float> d_coef;
   std::vector<float> h_coef;  // host mirror (ring sizing, FDN descriptors)
 
@@ -823,6 +825,8 @@ struct mlb_graph
   DevBuf<float> d_dmem;
   size_t dmem_floats = 0;
   std::vector<unsigned> ring_stride;  // per node, 0 = no ring
+  std::vector<std::pair<unsigned long long, unsigned>> dmem_lanes;  // (offset, floats per voice) of each row and ring
+  DevBuf<unsigned char> d_reset;  // staging of mlb_graph_reset_voices
 
   // chain scheduler words, all maintained by the kernels themselves (see ChainArgs)
   DevBuf<unsigned> d_sched;
@@ -1385,23 +1389,27 @@ extern "C" int mlb_graph_create(const mlb_node* nodes, int n_nodes, const int32_
 
   const size_t V = (size_t)n_voices;
   MLB_TRY(g->d_state.alloc(std::max<size_t>(1, lay.n_state_words) * V * 4, "voice state"));
+  MLB_TRY(g->d_state0.alloc(g->d_state.bytes(), "voice start state"));
   MLB_TRY(g->d_coef.alloc(std::max<size_t>(1, lay.n_coef_words) * V * 4, "voice coefficients"));
   // [0] unit counter, [1 + g] finished chunks of group g, [1 + G] finished units, [2 + G] progress base
   MLB_TRY(g->d_sched.alloc(((V + 31) / 32 + 3) * 4, "scheduler words"));
   CU_CHECK(cudaMemset(g->d_sched.get(), 0, g->d_sched.bytes()));
-  CU_CHECK(cudaMemset(g->d_state.get(), 0, g->d_state.bytes()));
-  // state of freshly constructed functors: zeros, except the "idle" markers
-  for (int i = 0; i < n_nodes; ++i)
+  // state of freshly constructed functors: zeros, except the "idle" markers; the start state too
+  for (uint32_t* st : {g->d_state.get(), g->d_state0.get()})
   {
-    int word = -1;
-    uint32_t val = 0;
-    if (nodes[i].op == MLB_OP_ADSR) word = 7, val = 4u;                   // segment{off}, F:694
-    if (nodes[i].op == MLB_OP_GLIDE) word = 2, val = 0xFFFFFFFFu;         // mVectorsRemaining{-1}, G:440
-    if (nodes[i].op == MLB_OP_SAMPLE_GLIDE) word = 3, val = 0xFFFFFFFFu;  // mSamplesRemaining{-1}, G:524
-    if (nodes[i].op == MLB_OP_TEMPO_LOCK) word = 0, val = 0xBF800000u;    // _omega{-1.f}, F:1481
-    if (word < 0) continue;
-    std::vector<uint32_t> fill(V, val);
-    CU_CHECK(cudaMemcpy(g->d_state.get() + (size_t)(so[i] + word) * V, fill.data(), V * 4, cudaMemcpyHostToDevice));
+    CU_CHECK(cudaMemset(st, 0, g->d_state.bytes()));
+    for (int i = 0; i < n_nodes; ++i)
+    {
+      int word = -1;
+      uint32_t val = 0;
+      if (nodes[i].op == MLB_OP_ADSR) word = 7, val = 4u;                   // segment{off}, F:694
+      if (nodes[i].op == MLB_OP_GLIDE) word = 2, val = 0xFFFFFFFFu;         // mVectorsRemaining{-1}, G:440
+      if (nodes[i].op == MLB_OP_SAMPLE_GLIDE) word = 3, val = 0xFFFFFFFFu;  // mSamplesRemaining{-1}, G:524
+      if (nodes[i].op == MLB_OP_TEMPO_LOCK) word = 0, val = 0xBF800000u;    // _omega{-1.f}, F:1481
+      if (word < 0) continue;
+      std::vector<uint32_t> fill(V, val);
+      CU_CHECK(cudaMemcpy(st + (size_t)(so[i] + word) * V, fill.data(), V * 4, cudaMemcpyHostToDevice));
+    }
   }
   CU_CHECK(cudaMemset(g->d_coef.get(), 0, g->d_coef.bytes()));
   g->h_coef.assign((size_t)lay.n_coef_words * V, 0.f);
@@ -1515,6 +1523,7 @@ static int size_functor_memory(mlb_graph* g)
   const int n = (int)g->nodes.size();
   std::vector<unsigned> stride(n, 0u);
   std::vector<unsigned long long> row_off(n, 0ull), ring_off(n, 0ull);
+  std::vector<std::pair<unsigned long long, unsigned>> lanes;
   unsigned long long total = 0;
   for (int i = 0; i < n; ++i)
   {
@@ -1530,6 +1539,7 @@ static int size_functor_memory(mlb_graph* g)
     if (rows)
     {
       row_off[i] = total;
+      lanes.emplace_back(total, (unsigned)MLB_BLOCK);
       total += (unsigned long long)V * MLB_BLOCK;
     }
     if (rings)
@@ -1552,6 +1562,7 @@ static int size_functor_memory(mlb_graph* g)
       while (ring < (unsigned)(dmax + MLB_BLOCK)) ring <<= 1;
       stride[i] = ring;
       ring_off[i] = total;
+      lanes.emplace_back(total, ring);
       total += (unsigned long long)V * ring;
     }
   }
@@ -1563,6 +1574,7 @@ static int size_functor_memory(mlb_graph* g)
   MLB_TRY(g->d_dmem.alloc(std::max<unsigned long long>(total, 1) * 4, "delay memory"));
   g->dmem_floats = (size_t)total;
   g->ring_stride = stride;
+  g->dmem_lanes = lanes;
   for (GNode& gn : g->gnodes)
   {
     if (gn.src_node < 0) continue;
@@ -1600,8 +1612,10 @@ extern "C" int mlb_graph_set_state(mlb_graph* g, const uint32_t* state_host)
   if (!g) return fail(MLB_ERR_INVALID, "null graph");
   if (g->layout.n_state_words == 0) return MLB_OK;
   if (!state_host) return fail(MLB_ERR_INVALID, "null state");
-  CU_CHECK(cudaMemcpy(g->d_state.get(), state_host, (size_t)g->layout.n_state_words * g->V * 4,
-                      cudaMemcpyHostToDevice));
+  // both copies from the host: each cudaMemcpy has finished when it returns, so a later reset on the graph's stream
+  // reads the new start state
+  for (uint32_t* st : {g->d_state.get(), g->d_state0.get()})
+    CU_CHECK(cudaMemcpy(st, state_host, (size_t)g->layout.n_state_words * g->V * 4, cudaMemcpyHostToDevice));
   return MLB_OK;
 }
 extern "C" int mlb_graph_get_state(mlb_graph* g, uint32_t* state_host)
@@ -2345,8 +2359,10 @@ struct mlb_voices
   float gl_per = 0.f, gl_dy = 0.f, dr_per = 0.f, dr_dy = 0.f, pc_per = 0.f, pc_dy = 0.f;
   unsigned flags = 0;
   DevBuf<uint32_t> d_state;
+  DevBuf<uint32_t> d_state0;  // the words mlb_voices_create wrote: a voice's start state
   DevBuf<float> d_coef, d_grows;
   DevBuf<int32_t> d_main;  // MPE: index of each voice's main voice, or -1
+  DevBuf<unsigned char> d_reset;  // staging of mlb_voices_reset
   DevBuf<mlb_voice_events> d_ev;
   DevBuf<float> d_out;
 };
@@ -2407,9 +2423,11 @@ extern "C" int mlb_voices_create(int n_voices, float sample_rate, const int32_t*
     co[(size_t)VC_VOICE_ROW * V + v] = (float)voice_index[v] - 1;   // :292
   }
   MLB_TRY(vb->d_state.alloc(st.size() * 4, "voice bank"));
+  MLB_TRY(vb->d_state0.alloc(st.size() * 4, "voice bank"));
   MLB_TRY(vb->d_coef.alloc(co.size() * 4, "voice bank"));
   MLB_TRY(vb->d_grows.alloc((size_t)VG_COUNT * V * MLB_BLOCK * 4, "voice bank"));
   CU_CHECK(cudaMemcpy(vb->d_state.get(), st.data(), st.size() * 4, cudaMemcpyHostToDevice));
+  CU_CHECK(cudaMemcpy(vb->d_state0.get(), st.data(), st.size() * 4, cudaMemcpyHostToDevice));
   CU_CHECK(cudaMemcpy(vb->d_coef.get(), co.data(), co.size() * 4, cudaMemcpyHostToDevice));
   CU_CHECK(cudaMemset(vb->d_grows.get(), 0, vb->d_grows.bytes()));
   MLB_TRY(vb->stream.create(cudaStreamNonBlocking));
@@ -2706,6 +2724,7 @@ struct ListBank
   DevBuf<int32_t> d_vmap;  // [G + 2] offsets, then [V] voices grouped by instrument, the unmapped ones last
   DevBuf<int32_t> d_off;   // staging of the host entry points
   DevBuf<float> d_out;
+  DevBuf<unsigned char> d_reset;  // staging of the reset entry points
 };
 
 // The kernel arguments CtrlArgs and PtArgs share: the list's offsets, the output and the rows the bank writes.
@@ -2987,6 +3006,7 @@ extern "C" int mlb_synth_process_controllers_host(mlb_voices* vb, mlb_controller
 struct mlb_process_time : ListBank
 {
   DevBuf<uint64_t> d_state;    // [MLB_PT_WORDS][G]
+  DevBuf<uint64_t> d_state0;   // the words mlb_process_time_create wrote: an instrument's start state
   DevBuf<mlb_transport> d_tr;  // staging of the host entry points
 };
 
@@ -3012,6 +3032,7 @@ extern "C" int mlb_process_time_create(int n_instruments, double sample_rate, ml
   pt->G = n_instruments;
   const size_t G = (size_t)n_instruments;
   MLB_TRY(pt->d_state.alloc((size_t)MLB_PT_WORDS * G * 8, "process-time bank"));
+  MLB_TRY(pt->d_state0.alloc((size_t)MLB_PT_WORDS * G * 8, "process-time bank"));
   // ProcessTime's member defaults (MLAudioContext.h:43-56), then AudioContext::setSampleRate
   std::vector<uint64_t> st((size_t)MLB_PT_WORDS * G, 0u);
   const double ppq1 = -1.;
@@ -3021,6 +3042,7 @@ extern "C" int mlb_process_time_create(int n_instruments, double sample_rate, ml
   std::fill_n(st.begin() + MLB_PT_PPQ_POS1 * G, G, ppq1_bits);
   std::fill_n(st.begin() + MLB_PT_SAMPLE_RATE * G, G, sr_bits);
   CU_CHECK(cudaMemcpy(pt->d_state.get(), st.data(), st.size() * 8, cudaMemcpyHostToDevice));
+  CU_CHECK(cudaMemcpy(pt->d_state0.get(), st.data(), st.size() * 8, cudaMemcpyHostToDevice));
   MLB_TRY(pt->stream.create(cudaStreamNonBlocking));
   *out = pt.release();
   return MLB_OK;
@@ -3109,6 +3131,7 @@ struct mlb_routers
   DevBuf<mlb_event> d_ev;
   DevBuf<mlb_voice_events> d_rec;
   DevBuf<mlb_controller_change> d_ch;
+  DevBuf<unsigned char> d_reset;  // staging of mlb_routers_reset
 };
 
 extern "C" int mlb_routers_destroy(mlb_routers* r)
@@ -3312,6 +3335,7 @@ struct mlb_published
   DevBuf<uint32_t> d_state;  // [n_signals][G][3]
   DevBuf<float> d_dest;      // staging of mlb_published_read_host
   DevBuf<int32_t> d_counts;
+  DevBuf<unsigned char> d_reset;  // staging of mlb_published_reset
 };
 
 extern "C" int mlb_published_destroy(mlb_published* p)
@@ -3652,6 +3676,135 @@ extern "C" int mlb_synth_process_published_host(mlb_routers* r, mlb_voices* vb, 
   if (!p) return fail(MLB_ERR_INVALID, "null published bank");
   return synth_routed(r, vb, cb, pt, g, b, p, offsets_host, events_host, n_events, time_offsets_host, transports_host,
                       n_transports, nullptr, nullptr, bus_host, n_blocks);
+}
+
+// ------------------------------------------------------------------------------------------
+// Restart: the lane-selective resets (restart_kernel.cuh, DESIGN.md "Restart")
+
+// The checks of every mlb_*_reset, all before anything is written: a list of n >= 0 indexes (null only when n is 0), a
+// bank, and every index in [0, limit).
+static int reset_check(const void* bank, const char* what, const int32_t* list, int n, int limit, const char* unit)
+{
+  if (n < 0) return fail(MLB_ERR_INVALID, "%s reset: n must not be negative (got %d)", what, n);
+  if (n > 0 && !list) return fail(MLB_ERR_INVALID, "%s reset: null %s list of %d entries", what, unit, n);
+  if (!bank) return fail(MLB_ERR_INVALID, "null %s", what);
+  for (int i = 0; i < n; ++i)
+    if (list[i] < 0 || list[i] >= limit)
+      return fail(MLB_ERR_INVALID, "%s reset: %s %d (list index %d) is not in 0..%d", what, unit, list[i], i, limit - 1);
+  return MLB_OK;
+}
+
+// Sets the regions of the distinct lanes of `list` in one launch of reset_lanes_kernel on `stream` and returns when it
+// has run.  The regions and the lanes go up in one copy through `staging`.  An empty list or no regions: nothing.
+static int reset_lanes(cudaStream_t stream, DevBuf<unsigned char>& staging, const std::vector<ResetRegion>& regions,
+                       const int32_t* list, int n)
+{
+  if (n == 0 || regions.empty()) return MLB_OK;
+  std::vector<int32_t> lanes(list, list + n);
+  std::sort(lanes.begin(), lanes.end());
+  lanes.erase(std::unique(lanes.begin(), lanes.end()), lanes.end());
+  const size_t rb = regions.size() * sizeof(ResetRegion), lb = lanes.size() * sizeof(int32_t);
+  std::vector<unsigned char> up(rb + lb);
+  memcpy(up.data(), regions.data(), rb);
+  memcpy(up.data() + rb, lanes.data(), lb);
+  MLB_TRY(staging.ensure(up.size(), "staging"));
+  const long long items = (long long)lanes.size() * (long long)regions.size();
+  const auto* d_regions = reinterpret_cast<const ResetRegion*>(staging.get());
+  const auto* d_lanes = reinterpret_cast<const int32_t*>(staging.get() + rb);
+  CU_CHECK(cudaMemcpyAsync(staging.get(), up.data(), up.size(), cudaMemcpyHostToDevice, stream));
+  reset_lanes_kernel<<<(unsigned)((items + kResetWarps - 1) / kResetWarps), 32 * kResetWarps, 0, stream>>>(
+      d_regions, (int)regions.size(), d_lanes, items);
+  ++g_launches;
+  CU_CHECK(cudaGetLastError());
+  CU_CHECK(cudaStreamSynchronize(stream));
+  return MLB_OK;
+}
+
+// an SoA word array [rows][N] (32-bit words), column = lane
+static ResetRegion soa_region(void* dst, const void* src, uint32_t fill, int rows, size_t N)
+{
+  return {static_cast<uint32_t*>(dst), static_cast<const uint32_t*>(src), fill, rows, 1, (long long)N, 1};
+}
+// `words` zero words per lane at dst + lane * pitch (+ k * row_pitch for each of `rows` rows)
+static ResetRegion zero_region(void* dst, int rows, int words, long long row_pitch, long long pitch)
+{
+  return {static_cast<uint32_t*>(dst), nullptr, 0u, rows, words, row_pitch, pitch};
+}
+
+extern "C" int mlb_graph_reset_voices(mlb_graph* g, const int32_t* voices, int n)
+{
+  MLB_TRY(reset_check(g, "graph", voices, n, g ? g->V : 0, "voice"));
+  const size_t V = (size_t)g->V;
+  std::vector<ResetRegion> r;
+  if (g->layout.n_state_words) r.push_back(soa_region(g->d_state.get(), g->d_state0.get(), 0u, g->layout.n_state_words, V));
+  // the delay memory: every row and ring of the voice (the write index is global and stays: DESIGN.md "Restart")
+  if (g->d_dmem.get())
+    for (const auto& seg : g->dmem_lanes) r.push_back(zero_region(g->d_dmem.get() + seg.first, 1, (int)seg.second, 0, seg.second));
+  if (g->d_ring.get())
+  {
+    r.push_back(zero_region(g->d_ring.get(), 1, 8 * g->ring_len, 0, 8ll * g->ring_len));
+    r.push_back(zero_region(g->d_carry.get(), 1, 8 * MLB_BLOCK, 0, 8 * MLB_BLOCK));
+  }
+  return reset_lanes(g->stream.get(), g->d_reset, r, voices, n);
+}
+
+extern "C" int mlb_voices_reset(mlb_voices* vb, const int32_t* voices, int n)
+{
+  MLB_TRY(reset_check(vb, "voice bank", voices, n, vb ? vb->V : 0, "voice"));
+  const size_t V = (size_t)vb->V;
+  const std::vector<ResetRegion> r = {soa_region(vb->d_state.get(), vb->d_state0.get(), 0u, VS_COUNT, V),
+                                      zero_region(vb->d_grows.get(), VG_COUNT, MLB_BLOCK, (long long)V * MLB_BLOCK,
+                                                  MLB_BLOCK)};
+  return reset_lanes(vb->stream.get(), vb->d_reset, r, voices, n);
+}
+
+extern "C" int mlb_routers_reset(mlb_routers* r, const int32_t* instruments, int n)
+{
+  MLB_TRY(reset_check(r, "router bank", instruments, n, r ? r->G : 0, "instrument"));
+  // what router_clear_kernel zeroes, for the listed instruments: every word but the two counters
+  static_assert(RW_SCALAR == RW_OVERFLOW + 1 && RW_SCALAR == kRouterWords - 1, "the counter rows are the last two");
+  uint32_t* st = r->d_state.get();
+  const long long pitch = kRouterWords * 32;
+  const std::vector<ResetRegion> reg = {
+      zero_region(st, 1, RW_OVERFLOW * 32, 0, pitch),
+      zero_region(st + RW_SCALAR * 32, 1, RS_UNSUPPORTED, 0, pitch),
+      zero_region(st + RW_SCALAR * 32 + RS_UNSUPPORTED + 1, 1, 32 - RS_UNSUPPORTED - 1, 0, pitch)};
+  return reset_lanes(r->stream.get(), r->d_reset, reg, instruments, n);
+}
+
+extern "C" int mlb_controllers_reset(mlb_controllers* cb, const int32_t* instruments, int n)
+{
+  MLB_TRY(reset_check(cb, "controller bank", instruments, n, cb ? cb->G : 0, "instrument"));
+  // what mlb_controllers_clear writes, for the listed instruments
+  const size_t G = (size_t)cb->G, CG = (size_t)cb->C * G;
+  std::vector<ResetRegion> r;
+  for (int w = 0; w < CS_COUNT; ++w)
+    r.push_back(soa_region(cb->d_state.get() + w * CG, nullptr, w == CS_REM ? 0xFFFFFFFFu : 0u, cb->C, G));
+  r.push_back(zero_region(cb->d_rows.get(), cb->C, MLB_BLOCK, (long long)G * MLB_BLOCK, MLB_BLOCK));
+  return reset_lanes(cb->stream.get(), cb->d_reset, r, instruments, n);
+}
+
+extern "C" int mlb_process_time_reset(mlb_process_time* pt, const int32_t* instruments, int n)
+{
+  MLB_TRY(reset_check(pt, "process-time bank", instruments, n, pt ? pt->G : 0, "instrument"));
+  // [MLB_PT_WORDS][G] 64-bit words: two 32-bit words per instrument and row
+  const ResetRegion r = {reinterpret_cast<uint32_t*>(pt->d_state.get()),
+                         reinterpret_cast<const uint32_t*>(pt->d_state0.get()), 0u, MLB_PT_WORDS, 2,
+                         2ll * pt->G, 2};
+  return reset_lanes(pt->stream.get(), pt->d_reset, {r}, instruments, n);
+}
+
+extern "C" int mlb_published_reset(mlb_published* p, const int32_t* instruments, int n)
+{
+  MLB_TRY(reset_check(p, "published bank", instruments, n, p ? p->G : 0, "instrument"));
+  const int S = (int)p->signals.size();
+  std::vector<ResetRegion> r = {zero_region(p->d_state.get(), S, 3, 3ll * p->G, 3)};
+  for (int s = 0; s < S; ++s)
+  {
+    const PubSignal& sg = p->args.sig[s];
+    r.push_back(zero_region(p->d_ring.get() + sg.ring, 1, sg.size, 0, sg.size));
+  }
+  return reset_lanes(p->stream.get(), p->d_reset, r, instruments, n);
 }
 
 // ------------------------------------------------------------------------------------------
