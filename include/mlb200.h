@@ -859,6 +859,20 @@ int mlb_synth_process_published_host(mlb_routers* r, mlb_voices* vb, mlb_control
                                      const mlb_event* events_host, int n_events, const int32_t* time_offsets_host,
                                      const mlb_transport* transports_host, int n_transports, float* bus_host,
                                      int n_blocks);
+/* A synth whose Synth::processVector puts an instrument section after the voice sum (DESIGN.md "Instrument stage"):
+ * mlb_synth_process_published_host (p may be null), and per time chunk, after the graph, one assembly kernel writes
+ * the input planes of `gi`, a graph over the G instruments of the buses: [P + C + phase] planes per block, the P bus
+ * sums (the graph's audio outputs, summed as the bus sum does), then bit copies of the C controller planes and the
+ * beat-phase plane from each bus's first voice.  After K14 if p, gi runs on them, and bus_host [T][gi's outputs][G][64]
+ * receives its outputs.  MLB_ERR_INVALID, before anything is copied, also when gi is null, its lanes are not r's
+ * instruments, the buses are not r's instruments or one has no voice, or a gi INPUT plane is not within P + C + phase.
+ * P is taken from g (its outputs less p's planes); buses carry no plane count, so the caller builds gi for that P: a
+ * gi built for another P whose planes stay below P + C + phase is not caught and reads the wrong planes. */
+int mlb_synth_process_instrument_host(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb, mlb_process_time* pt,
+                                      mlb_graph* g, mlb_buses* b, mlb_published* p, mlb_graph* gi,
+                                      const int32_t* offsets_host, const mlb_event* events_host, int n_events,
+                                      const int32_t* time_offsets_host, const mlb_transport* transports_host,
+                                      int n_transports, float* bus_host, int n_blocks);
 
 /* ---- Restart: lane-selective resets (DESIGN.md "Restart") ----
  * Each sets the listed voices (graph, Voice bank) or instruments (the other banks) to the state a freshly

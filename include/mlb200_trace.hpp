@@ -39,7 +39,9 @@
 //
 // Header only; link against libmlb200.so.  No sample arithmetic happens on the CPU here.
 #pragma once
+#include <algorithm>
 #include <array>
+#include <climits>
 #include <cmath>
 #include <cstdint>
 #include <cstdio>
@@ -99,6 +101,17 @@ class Recorder
   // TracedSynth::trace: the one pass whose symbols may be read stale (pass 1 of this voice, while pass 2 runs); -2:
   // none.  -1 (TracedProcessor): any earlier pass.
   int staleEpoch = -1;
+  // TracedSynth::trace: the epochs of processVoice's passes, [voiceEpoch0, voiceEpoch1), and whether this recorder
+  // traces the instrument section (Synth::processVector around the base call) rather than processVoice
+  int voiceEpoch0 = 0, voiceEpoch1 = INT_MAX;
+  bool instrument = false;
+
+  // epochs are unique across recorders, so that a symbol of one recorder is never current in another
+  static int& lastEpoch()
+  {
+    static thread_local int e = 0;
+    return e;
+  }
 
   static Recorder*& current()
   {
@@ -113,7 +126,7 @@ class Recorder
   }
   void beginPass()
   {
-    ++epoch;
+    epoch = ++lastEpoch();
     nodes.clear();
     outs.clear();
     opCounter = 0;
@@ -209,14 +222,36 @@ class DSPVector
     // a symbol of the previous pass: state the caller keeps between process calls
     if (r.staleEpoch != -1)
     {
+      const bool ofVoice = epoch >= r.voiceEpoch0 && epoch < r.voiceEpoch1;
+      if (r.instrument)
+      {
+        if (ofVoice)
+          throw Error(MLB_ERR_UNSUPPORTED,
+                      "mlb::tr::TracedSynth: Synth::processVector reads, outside the base Synth::processVector call, a "
+                      "DSPVector made in processVoice (a Voice& kept past the call, or a voice's member); the instrument "
+                      "section sees the voices only through the bus rows the base call leaves in its outputs");
+        if (epoch != r.staleEpoch)
+          throw Error(MLB_ERR_UNSUPPORTED,
+                      "mlb::tr::TracedSynth: Synth::processVector reads a DSPVector made before this trace");
+        if (opIndex < 0)
+          throw Error(MLB_ERR_UNSUPPORTED,
+                      "mlb::tr::TracedSynth: Synth::processVector carries a bus row, controller, beat phase or tr::param "
+                      "between vectors as it stands; carry an expression of it (e.g. row * 1.f)");
+      }
+      else if (!ofVoice)
+        throw Error(MLB_ERR_UNSUPPORTED,
+                    ("mlb::tr::TracedSynth: voice " + std::to_string(r.voice) +
+                     " reads a DSPVector made outside processVoice (before the base Synth::processVector call, or by "
+                     "the instrument section); processVoice may read only its own rows, controllers and members")
+                        .c_str());
       // a voice's own member is written only in its own two passes; anything older was written by another voice
-      if (epoch != r.staleEpoch)
+      else if (epoch != r.staleEpoch)
         throw Error(MLB_ERR_UNSUPPORTED,
                     ("mlb::tr::TracedSynth: voice " + std::to_string(r.voice) +
                      " reads a DSPVector of another voice (a member shared between voices, or another voice's Voice "
                      "rows); a row carried between vectors must be per voice, e.g. DSPVector carried[16]")
                         .c_str());
-      if (opIndex < 0)
+      else if (opIndex < 0)
         throw Error(MLB_ERR_UNSUPPORTED,
                     ("mlb::tr::TracedSynth: voice " + std::to_string(r.voice) +
                      " carries a Voice row, controller, beat phase or tr::param between vectors as it stands; carry "
@@ -247,6 +282,11 @@ inline DSPVector op3(int op, const DSPVector& a, const DSPVector& b, const DSPVe
 inline DSPVector param(const char* name, float value)
 {
   Recorder& r = Recorder::get();
+  if (r.instrument)
+    throw Error(MLB_ERR_UNSUPPORTED, (std::string("mlb::tr::TracedSynth: tr::param(") + name + ") in Synth::processVector "
+                                     "outside the base call: the instrument section has no per-instrument parameters "
+                                     "(TracedSynth::setParam sets the voices' only); use a float or a controller")
+                                        .c_str());
   const int n = r.addNode(MLB_OP_PARAM, {}, 0, false);
   r.nodes[(size_t)n].coef[0] = value;
   r.nodes[(size_t)n].name = name;
@@ -561,6 +601,11 @@ class Functor
     {
       // in the reference one object shared by two voices ticks once per voice and vector; each lane here has its own
       auto it = r.functorVoice->emplace(this, r.voice).first;
+      if (it->second != r.voice && (it->second < 0 || r.voice < 0))  // -1: the instrument section
+        throw Error(MLB_ERR_UNSUPPORTED, ("mlb::tr: a functor object is called by voice " +
+                                          std::to_string(std::max(it->second, r.voice)) + " and by the instrument "
+                                          "section of Synth::processVector; each needs its own")
+                                             .c_str());
       if (it->second != r.voice)
         throw Error(MLB_ERR_UNSUPPORTED, ("mlb::tr: a functor object is called by voice " + std::to_string(it->second) +
                                           " and voice " + std::to_string(r.voice) + "; each voice needs its own")
@@ -1446,12 +1491,16 @@ using Symbol = std::string;  // what setInputProtocol takes ("MIDI" or "MPE")
 // MLSynth.h:16-19, a host scalar
 inline float pitchToFrequency(float pitch) { return 440.0f * powf(2.0f, (pitch - 69.0f) / 12.0f); }
 
-// what getInputVoice / getInputController / getBeatPhase return while TracedSynth::trace runs one voice
+// what getInputVoice / getInputController / getBeatPhase return while TracedSynth::trace runs one voice, or (voice -1)
+// the instrument section of Synth::processVector
 struct SynthPass
 {
   static constexpr int kPhasePlane = 1 << 20;  // INPUT iarg of the beat phase until the controller count is known
   static constexpr int kAccPlane = 1 << 21;    // INPUT iarg kAccPlane + i: the accumulator outputs[i] at entry
+  static constexpr int kBusPlane = 1 << 22;    // instrument section: kBusPlane + i, bus row i after the base call
+  static constexpr int kOutPlane = 1 << 23;    // instrument section: kOutPlane + i, outputs[i] at entry
   int voice = -1;
+  std::function<void(DSPVectorDynamic&)> base;  // instrument section: what the base Synth::processVector does
   EventsToSignals::Voice rows;
   std::vector<int>* controllers = nullptr;  // controller numbers in first-use order, over all voices
   std::map<int, int> controllerNode;        // this pass: controller number -> its INPUT node
@@ -1497,6 +1546,11 @@ class AudioContext
   const EventsToSignals::Voice& getInputVoice(int n)
   {
     if (!pass_) throw Error(MLB_ERR_INVALID, "mlb::tr: getInputVoice outside TracedSynth::trace()");
+    if (pass_->voice < 0)
+      throw Error(MLB_ERR_UNSUPPORTED, ("mlb::tr::TracedSynth: getInputVoice(" + std::to_string(n) + ") outside the base "
+                                        "Synth::processVector call; the instrument section sees the voices only through "
+                                        "the bus rows the base call leaves in its outputs")
+                                           .c_str());
     if (n != pass_->voice)
       throw Error(MLB_ERR_UNSUPPORTED, ("mlb::tr: voice " + std::to_string(pass_->voice) + " reads the rows of voice " +
                                         std::to_string(n) + "; a voice may read only its own rows")
@@ -1587,7 +1641,10 @@ class SignalProcessor
     if (s == (int)published_.size()) return;
     const PublishDecl& d = published_[(size_t)s];
     const std::string what = "mlb::tr: storePublishedSignal(" + signalName + "): ";
-    if (!publishStores_) throw Error(MLB_ERR_INVALID, (what + "outside TracedSynth::trace()").c_str());
+    if (!publishStores_)
+      throw Error(inSynthTrace_ ? MLB_ERR_UNSUPPORTED : MLB_ERR_INVALID,
+                  (what + (inSynthTrace_ ? "outside processVoice; only a voice publishes" : "outside TracedSynth::trace()"))
+                      .c_str());
     if ((int)CHANNELS != d.channels)
       throw Error(MLB_ERR_UNSUPPORTED, (what + "a DSPVectorArray<" + std::to_string(CHANNELS) + "> into a signal of " +
                                         std::to_string(d.channels) + " channels (the reference's rotate buffer would be "
@@ -1623,6 +1680,7 @@ class SignalProcessor
   friend class TracedSynth;
   std::vector<PublishDecl> published_;
   std::vector<PublishStore>* publishStores_ = nullptr;  // set by TracedSynth::trace while processVoice runs
+  bool inSynthTrace_ = false;                           // set by TracedSynth::trace for the whole trace
 };
 
 // Synth (MLSynth.h:26-93): subclasses implement processVoice; TracedSynth traces it once per voice
@@ -1639,6 +1697,11 @@ class Synth : public SignalProcessor
   {
     auto* audioContext = static_cast<AudioContext*>(stateData);
     if (!audioContext) return;
+    if (audioContext->pass_ && audioContext->pass_->base)  // TracedSynth::trace: every voice, then the bus rows
+    {
+      audioContext->pass_->base(outputs);
+      return;
+    }
     for (int i = 0; i < (int)outputs.size(); ++i) outputs[i] = DSPVector{0.f};
     int activeCount = 0;
     for (int v = 0; v < numVoices_; ++v)
@@ -1874,7 +1937,12 @@ class TracedProcessor
 // instrument as ((+0 + x0) + x1) + ..., which is what Synth::processVector's `outputs[i] = 0; outputs[i] += ...` gives
 // in voice order.  All voices must record the same nodes; their coefficient and state words may differ (a cutoff
 // that depends on voiceIndex) and become per-lane words.  The graph's INPUT planes follow contract E: the Voice rows
-// at 0..7, the controllers a voice reads at 8 + k in first-use order, the beat phase after them.
+// at 0..7, the controllers at 8 + k in first-use order, the beat phase after them.
+//
+// processVoice runs inside the base Synth::processVector, which trace() reaches through synth.processVector.  An
+// override that calls the base once and works on the bus rows it leaves (an effects section per instrument) becomes a
+// second graph, over instrument lanes, on the bus rows, the controllers and the beat phase (DESIGN.md, "Instrument
+// stage"); a synth without such a section builds none.
 class TracedSynth
 {
   struct VoiceGraph
@@ -1883,7 +1951,15 @@ class TracedSynth
     std::vector<int32_t> outs;
     std::vector<PublishStore> stores;  // rows: nodes of this graph
   };
+  struct InstrumentGraph
+  {
+    std::vector<TNode> nodes;  // none: Synth::processVector is the base's, its outputs the bus rows
+    std::vector<int32_t> outs;
+    int planes = 0;  // INPUT planes: the bus rows, the controllers, the beat phase
+  };
   std::vector<VoiceGraph> voices_;  // one per synth voice
+  InstrumentGraph instrument_;
+  size_t busPlanes_ = 0;  // the outputs Synth::processVector hands to the base call
   std::vector<mlb_node> nodes_;
   std::vector<int32_t> outs_;
   std::vector<PublishDecl> published_;  // the synth's publishSignal declarations
@@ -1903,6 +1979,7 @@ class TracedSynth
   std::unique_ptr<Buses> buses_;
   std::unique_ptr<DeviceBank> bank_;  // the graph over every lane
   std::unique_ptr<PublishedBank> pubBank_;
+  std::unique_ptr<DeviceBank> ibank_;  // the instrument graph over the instruments, if there is one
   std::vector<int64_t> overflow_;  // the router bank's overflow counts after the last call
 
   DeviceBank& bank() const
@@ -1982,22 +2059,108 @@ class TracedSynth
       const mlb_node& m = rec.nodes[(size_t)j].node;
       if (m.op == MLB_OP_INPUT && m.iarg < MLB_VOICE_ROWS && uses[(size_t)j] == 0) drop[(size_t)j] = 1;
     }
-    std::vector<int> idx((size_t)n, -1);
     VoiceGraph vg;
-    for (int j = 0; j < n; ++j)
-      if (!drop[(size_t)j]) idx[(size_t)j] = (int)vg.nodes.size(), vg.nodes.push_back(rec.nodes[(size_t)j]);
-    for (TNode& t : vg.nodes)
+    const std::vector<int> idx = keepNodes(rec.nodes, drop, vg.nodes);
+    for (int i = 0; i < nOut; ++i) vg.outs.push_back(x[(size_t)i] < 0 ? -1 : idx[(size_t)x[(size_t)i]]);
+    for (PublishStore& st : stores)
+      for (int& s : st.rows) s = idx[(size_t)s];
+    vg.stores = std::move(stores);
+    return vg;
+  }
+
+  // the nodes not dropped, renumbered (operands, feedback writes, further calls); returns old index -> new (-1: dropped)
+  static std::vector<int> keepNodes(const std::vector<TNode>& nodes, const std::vector<char>& drop, std::vector<TNode>& kept)
+  {
+    std::vector<int> idx(nodes.size(), -1);
+    for (size_t j = 0; j < nodes.size(); ++j)
+      if (!drop[j]) idx[j] = (int)kept.size(), kept.push_back(nodes[j]);
+    for (TNode& t : kept)
     {
       for (int k = 0; k < MLB_MAX_INS; ++k)
         if (t.node.in[k] >= 0) t.node.in[k] = idx[(size_t)t.node.in[k]];
       if (t.node.op == MLB_OP_FEEDBACK_WRITE) t.node.iarg = idx[(size_t)t.node.iarg];
       else if (isAgain(t.node)) t.node.iarg = MLB_AGAIN(idx[(size_t)MLB_AGAIN_TARGET(t.node.iarg)]);
     }
-    for (int i = 0; i < nOut; ++i) vg.outs.push_back(x[(size_t)i] < 0 ? -1 : idx[(size_t)x[(size_t)i]]);
-    for (PublishStore& st : stores)
-      for (int& s : st.rows) s = idx[(size_t)s];
-    vg.stores = std::move(stores);
-    return vg;
+    return idx;
+  }
+
+  // The instrument section (Synth::processVector around the base call) as a graph over instrument lanes.  Its INPUT
+  // planes: the P bus rows, the C controllers, the beat phase.  No nodes when the section only hands `outputs` to the
+  // base call: the outputs are then the bus rows as they are.
+  static InstrumentGraph instrumentGraph(const Recorder& rec, size_t P, size_t nOut, size_t C, bool phase)
+  {
+    const std::string pv = "mlb::tr::TracedSynth: Synth::processVector ";
+    const int n = (int)rec.nodes.size();
+    const auto entry = [&](int j)  // i if node j is outputs[i] at entry (the reference's: the previous vector's), or -1
+    {
+      const mlb_node& m = rec.nodes[(size_t)j].node;
+      return m.op == MLB_OP_INPUT && m.iarg >= SynthPass::kOutPlane ? m.iarg - SynthPass::kOutPlane : -1;
+    };
+    const auto stale = [&](int i)
+    {
+      return Error(MLB_ERR_UNSUPPORTED, (pv + "reads outputs[" + std::to_string(i) + "] before assigning it; in the "
+                                              "reference it still holds the previous vector's output").c_str());
+    };
+    std::vector<int> uses((size_t)n, 0);
+    for (const TNode& t : rec.nodes)
+      for (int k = 0; k < MLB_MAX_INS; ++k)
+        if (t.node.in[k] >= 0)
+        {
+          if (entry(t.node.in[k]) >= 0) throw stale(entry(t.node.in[k]));
+          ++uses[(size_t)t.node.in[k]];
+        }
+    for (size_t i = 0; i < rec.outs.size(); ++i)
+    {
+      const int e = entry(rec.outs[i]);
+      if (e == (int)i)
+        throw Error(MLB_ERR_UNSUPPORTED,
+                    (pv + "leaves outputs[" + std::to_string(i) + "] unassigned: it is neither handed to the base "
+                          "Synth::processVector nor assigned after it, so in the reference it holds the previous "
+                          "vector's value").c_str());
+      if (e >= 0) throw stale(e);
+      ++uses[(size_t)rec.outs[i]];
+    }
+    std::vector<char> drop((size_t)n, 0);  // INPUT nodes nothing reads: outputs at entry, bus rows passed through
+    size_t kept = 0;
+    for (int j = 0; j < n; ++j)
+      kept += !(drop[(size_t)j] = rec.nodes[(size_t)j].node.op == MLB_OP_INPUT && uses[(size_t)j] == 0);
+    InstrumentGraph ig;
+    bool passThrough = P == nOut && kept == nOut;
+    for (size_t i = 0; i < nOut && passThrough; ++i)
+    {
+      const mlb_node& m = rec.nodes[(size_t)rec.outs[i]].node;
+      passThrough = m.op == MLB_OP_INPUT && m.iarg == SynthPass::kBusPlane + (int)i;
+    }
+    if (passThrough) return ig;
+    const std::vector<int> idx = keepNodes(rec.nodes, drop, ig.nodes);
+    for (TNode& t : ig.nodes)
+      if (t.node.op == MLB_OP_INPUT)
+        t.node.iarg = t.node.iarg == SynthPass::kPhasePlane ? (int)(P + C)
+                      : t.node.iarg >= SynthPass::kBusPlane ? t.node.iarg - SynthPass::kBusPlane
+                                                            : (int)P + t.node.iarg - MLB_VOICE_ROWS;
+    for (int32_t o : rec.outs) ig.outs.push_back(idx[(size_t)o]);
+    // an output that is an input row as it is, or that an earlier output already is, leaves through a copy of its own,
+    // select(x, x, x) (bitwise: exactly x): each graph output is a distinct node
+    std::vector<char> isOut(ig.nodes.size(), 0);
+    for (int32_t& o : ig.outs)
+    {
+      if (ig.nodes[(size_t)o].node.op == MLB_OP_INPUT || isOut[(size_t)o])
+      {
+        TNode c;
+        c.node.op = MLB_OP_SELECT;
+        for (int k = 0; k < MLB_MAX_INS; ++k) c.node.in[k] = k < 3 ? o : -1;
+        c.node.iarg = 0;
+        o = (int32_t)ig.nodes.size();
+        ig.nodes.push_back(c);
+        isOut.push_back(0);
+      }
+      isOut[(size_t)o] = 1;
+    }
+    ig.planes = (int)(P + C) + (phase ? 1 : 0);
+    std::vector<mlb_node> m;
+    for (const TNode& t : ig.nodes) m.push_back(t.node);
+    checkLayout(m);
+    return ig;
   }
 
   static bool sameStructure(const VoiceGraph& a, const VoiceGraph& b, std::string& where)
@@ -2055,22 +2218,30 @@ class TracedSynth
                       .c_str());
     if (ctx.input.modCC < 0 || ctx.input.modCC > 127)
       throw Error(MLB_ERR_INVALID, ("mlb::tr::TracedSynth: mod CC " + std::to_string(ctx.input.modCC) + " is not in 0..127").c_str());
-    Recorder rec;
+    Recorder rec, irec;  // processVoice's, and the instrument section's (Synth::processVector around the base call)
     std::map<const void*, int> functorVoice;
     std::vector<int> controllers;
     bool phase = false;
     std::vector<VoiceGraph> graphs;
     std::vector<SynthPass> passes((size_t)V);  // kept for the whole trace: a Voice& held by a later voice stays valid
     std::vector<PublishStore> stores;          // this pass's storePublishedSignal calls
+    SynthPass ipass;                           // the instrument section's: no voice
+    int ipassIndex = 0, baseCalls = 0;
+    size_t nBus = 0;             // the outputs handed to the base call: the bus rows
+    bool baseOnOutputs = false;  // the base call was handed `outputs` itself
+    const std::string pv = "mlb::tr::TracedSynth: Synth::processVector ";
+    // processVoice for every voice, two passes each, into `outputs` (what the base call was handed)
+    const auto traceVoices = [&](DSPVectorDynamic& outputs)
     {
       TraceScope scope(rec, ctx);
-      struct StoreSink  // where the synth's stores are recorded, for the lifetime of the trace
+      struct StoreSink  // where the synth's stores are recorded, while processVoice runs
       {
         SignalProcessor& sp;
         ~StoreSink() { sp.publishStores_ = nullptr; }
       } sink{synth};
       synth.publishStores_ = &stores;
       rec.functorVoice = &functorVoice;
+      rec.voiceEpoch0 = Recorder::lastEpoch() + 1;
       for (int v = 0; v < V; ++v)
       {
         SynthPass& pass = passes[(size_t)v];
@@ -2088,20 +2259,20 @@ class TracedSynth
           for (int r = 0; r < kNumVoiceOutputRows; ++r)
             pass.rows.outputs.row(r) = DSPVector::ofNode(rec.addNode(MLB_OP_INPUT, {}, r, false));
           acc.clear();
-          for (size_t i = 0; i < ctx.outputs.size(); ++i)
+          for (size_t i = 0; i < outputs.size(); ++i)
           {
             acc.push_back(rec.addNode(MLB_OP_INPUT, {}, SynthPass::kAccPlane + (int)i, false));
-            ctx.outputs[i] = DSPVector::ofNode(acc.back());
+            outputs[i] = DSPVector::ofNode(acc.back());
           }
           ctx.pass_ = &pass;
           if (!synth.isVoiceActive(v, ctx.getInputVoice(v)))
             refuse(v, "is not active (isVoiceActive returned false); every voice is processed on every vector");
-          synth.processVoice(v, ctx.getInputVoice(v), ctx.inputs, ctx.outputs, &ctx);
+          synth.processVoice(v, ctx.getInputVoice(v), ctx.inputs, outputs, &ctx);
           ctx.pass_ = nullptr;
         }
         rec.closeFeedback("processVoice");
         fin.clear();
-        for (size_t i = 0; i < ctx.outputs.size(); ++i) fin.push_back(ctx.outputs[i].resolve());
+        for (size_t i = 0; i < outputs.size(); ++i) fin.push_back(outputs[i].resolve());
         phase = phase || pass.phaseNode >= 0;
         graphs.push_back(extract(rec, acc, fin, v, stores));
         std::string where;
@@ -2109,7 +2280,63 @@ class TracedSynth
           refuse(v, "records a different graph from voice 0 (" + where +
                         "); voices may differ in coefficients and state only");
       }
+    };
+    // Synth::processVector, traced twice as TracedProcessor::trace does (carried members become feedback edges).  The
+    // base call leaves bus row i in its outputs[i]; in the second pass it first traces the voices, so that a voice
+    // reading what the first pass's instrument section left in a member is caught.  The controller planes follow
+    // first use in that second pass.
+    {
+      TraceScope scope(irec, ctx);
+      struct TraceFlag
+      {
+        SignalProcessor& sp;
+        ~TraceFlag() { sp.inSynthTrace_ = false; }
+      } flag{synth};
+      synth.inSynthTrace_ = true;
+      irec.instrument = true;
+      irec.voiceEpoch0 = irec.voiceEpoch1 = 0;  // no voice symbol exists until the base call traces the voices
+      irec.functorVoice = &functorVoice;
+      ipass.controllers = &controllers;
+      ipass.base = [&](DSPVectorDynamic& outputs)
+      {
+        if (++baseCalls > 1)
+          throw Error(MLB_ERR_UNSUPPORTED, (pv + "calls the base Synth::processVector more than once in a vector; it "
+                                                 "must call it exactly once").c_str());
+        if (ipassIndex == 0)
+          nBus = outputs.size(), baseOnOutputs = &outputs == &ctx.outputs;
+        else
+        {
+          if (outputs.size() != nBus || (&outputs == &ctx.outputs) != baseOnOutputs)
+            throw Error(MLB_ERR_INVALID, (pv + "is not deterministic between calls").c_str());
+          traceVoices(outputs);
+          irec.voiceEpoch0 = rec.voiceEpoch0, irec.voiceEpoch1 = Recorder::lastEpoch() + 1;
+        }
+        ctx.pass_ = &ipass;
+        for (size_t i = 0; i < outputs.size(); ++i)
+          outputs[i] = DSPVector::ofNode(irec.addNode(MLB_OP_INPUT, {}, SynthPass::kBusPlane + (int)i, false));
+      };
+      for (ipassIndex = 0; ipassIndex < 2; ++ipassIndex)
+      {
+        irec.staleEpoch = ipassIndex == 0 ? -2 : irec.epoch;
+        irec.beginPass();
+        baseCalls = 0;
+        controllers.clear();
+        ipass.controllerNode.clear();
+        ipass.phaseNode = -1;
+        for (size_t i = 0; i < ctx.outputs.size(); ++i)
+          ctx.outputs[i] = DSPVector::ofNode(irec.addNode(MLB_OP_INPUT, {}, SynthPass::kOutPlane + (int)i, false));
+        ctx.pass_ = &ipass;
+        synth.processVector(ctx.inputs, ctx.outputs, &ctx);
+        if (baseCalls == 0)
+          throw Error(MLB_ERR_UNSUPPORTED, (pv + "does not call the base Synth::processVector, which runs the voices; "
+                                                 "it must call it exactly once").c_str());
+      }
+      phase = phase || ipass.phaseNode >= 0;
+      ctx.pass_ = nullptr;
+      irec.closeFeedback("Synth::processVector");
+      for (size_t i = 0; i < ctx.outputs.size(); ++i) irec.outs.push_back(ctx.outputs[i].resolve());
     }
+    InstrumentGraph ig = instrumentGraph(irec, nBus, ctx.outputs.size(), controllers.size(), phase);
     // the beat phase after the controllers; untouched outputs read one shared +0 row
     const int phasePlane = MLB_VOICE_ROWS + (int)controllers.size();
     for (VoiceGraph& vg : graphs)
@@ -2151,6 +2378,8 @@ class TracedSynth
         }
     }
     published_ = synth.publishedSignals();
+    instrument_ = std::move(ig);
+    busPlanes_ = nBus;
     pubOuts_ = pubOuts;
     voices_ = std::move(graphs);
     controllers_ = controllers;
@@ -2172,6 +2401,9 @@ class TracedSynth
   const std::vector<PublishStore>& stores() const { return voices_.at(0).stores; }
   const std::vector<int32_t>& publishedOuts() const { return pubOuts_; }
   bool readsBeatPhase() const { return phase_; }
+  size_t outputs() const { return nOut_; }
+  size_t busPlanes() const { return busPlanes_; }
+  bool hasInstrumentGraph() const { return !instrument_.nodes.empty(); }
   const AudioContext::InputSettings& settings() const { return settings_; }
   int numVoices() const { return numVoices_; }
   // lanes of one instrument: polyphony voices, plus the MPE main voice first
@@ -2236,6 +2468,26 @@ class TracedSynth
       for (size_t i = 0; i < pubOuts_.size(); ++i) std::fprintf(f, "%s%d", i ? ", " : "", pubOuts_[i]);
       std::fprintf(f, "]");
     }
+    if (hasInstrumentGraph())  // the instrument section: its graph over instrument lanes, one set of words for all
+    {
+      const InstrumentGraph& ig = instrument_;
+      std::fprintf(f, ", \"instrument\": {\"planes\": %d, \"bus_planes\": %zu, \"nodes\": [", ig.planes, busPlanes_);
+      for (size_t i = 0; i < ig.nodes.size(); ++i)
+      {
+        const TNode& t = ig.nodes[i];
+        std::fprintf(f, "%s{\"op\": %d, \"in\": [", i ? ", " : "", t.node.op);
+        for (int k = 0; k < MLB_MAX_INS; ++k) std::fprintf(f, "%s%d", k ? ", " : "", t.node.in[k]);
+        std::fprintf(f, "], \"iarg\": %d, \"name\": \"%s\", \"coef\": [", t.node.iarg, t.name.c_str());
+        const bool again = isAgain(t.node);
+        if (!again) printWords(f, t.coef);
+        std::fprintf(f, "], \"state\": [");
+        if (!again) printWords(f, t.state);
+        std::fprintf(f, "]}");
+      }
+      std::fprintf(f, "], \"outs\": [");
+      for (size_t i = 0; i < ig.outs.size(); ++i) std::fprintf(f, "%s%d", i ? ", " : "", ig.outs[i]);
+      std::fprintf(f, "]}");
+    }
     std::fprintf(f, "}\n");
   }
 
@@ -2246,7 +2498,8 @@ class TracedSynth
   {
     if (nodes_.empty()) throw Error(MLB_ERR_INVALID, "mlb::tr::TracedSynth: trace() first");
     if (instruments < 1) throw Error(MLB_ERR_INVALID, "mlb::tr::TracedSynth: instruments must be positive");
-    pubBank_.reset(), bank_.reset(), buses_.reset(), times_.reset(), ctrl_.reset(), voiceBank_.reset(), routers_.reset();
+    ibank_.reset(), pubBank_.reset(), bank_.reset(), buses_.reset(), times_.reset(), ctrl_.reset(), voiceBank_.reset(),
+        routers_.reset();
     const AudioContext::InputSettings& s = settings_;
     const int G = instruments, NR = lanesPerInstrument(), V = G * NR;
     instruments_ = G, lanesPer_ = NR;
@@ -2291,6 +2544,15 @@ class TracedSynth
       for (const PublishStore& k : voices_[0].stores) st.push_back({k.signal, k.frames});
       pubBank_.reset(new PublishedBank(V, G, busFirst.data(), busCount.data(), sig, st));
     }
+    if (hasInstrumentGraph())
+    {
+      std::vector<mlb_node> in;
+      for (const TNode& t : instrument_.nodes) in.push_back(t.node);
+      ibank_.reset(new DeviceBank(in, instrument_.outs, G, flags));
+      for (size_t i = 0; i < in.size(); ++i)
+        for (int g = 0; g < G; ++g) loadWords(*ibank_, (int)i, g, instrument_.nodes[i]);
+      ibank_->commit();
+    }
     overflow_.assign((size_t)G, 0);
     for (size_t i = 0; i < nodes_.size(); ++i)
       for (int l = 0; l < V; ++l) loadWords(*bank_, (int)i, l, voices_[(size_t)laneVoice(l % NR)].nodes[i]);
@@ -2299,6 +2561,8 @@ class TracedSynth
   void commit() { bank().commit(); }
   int instruments() const { return instruments_; }
   const char* kernelName() const { return bank_ ? bank_->kernelName() : ""; }
+  // the instrument graph's kernel ("" without an instrument graph)
+  const char* instrumentKernelName() const { return ibank_ ? ibank_->kernelName() : ""; }
 
   // per-instrument, per-voice value of a tr::param(name, ...) scalar; call commit() after a batch of changes
   void setParam(const std::string& name, int instrument, int voice, float value)
@@ -2324,7 +2588,13 @@ class TracedSynth
                const mlb_transport* transports, int nTransports, float* bus, int nBlocks)
   {
     mlb_graph* graph = bank().handle();
-    if (pubBank_ && pubBank_->planes() > 0)  // K14 after the bus sum in every time chunk
+    if (ibank_)  // the instrument graph on the bus sums in every time chunk (K14 before it)
+      check(mlb_synth_process_instrument_host(
+          routers_->handle(), voiceBank_->handle(), ctrl_ ? ctrl_->handle() : nullptr, times_ ? times_->handle() : nullptr,
+          graph, buses_->handle(), pubBank_ && pubBank_->planes() > 0 ? pubBank_->handle() : nullptr, ibank_->handle(),
+          offsets, events, nEvents, times_ ? timeOffsets : nullptr, times_ ? transports : nullptr,
+          times_ ? nTransports : 0, bus, nBlocks));
+    else if (pubBank_ && pubBank_->planes() > 0)  // K14 after the bus sum in every time chunk
       check(mlb_synth_process_published_host(
           routers_->handle(), voiceBank_->handle(), ctrl_ ? ctrl_->handle() : nullptr, times_ ? times_->handle() : nullptr,
           graph, buses_->handle(), pubBank_->handle(), offsets, events, nEvents, times_ ? timeOffsets : nullptr,
@@ -2354,7 +2624,7 @@ class TracedSynth
   // synths[g] = make_unique<...>(..)`), fed only the events and transport updates from then on; the others are
   // untouched, bit for bit.  The graph lanes go back to the words of the last commit(), so setParam values stay.  One
   // launch per bank that holds state (routers, Voice rows, controllers and beat phase if built, graph, published
-  // signals if built), none for an empty list; an instrument out of range throws before anything is written.
+  // signals and instrument graph if built), none for an empty list; an instrument out of range throws before anything is written.
   void restart(const std::vector<int>& instruments)
   {
     DeviceBank& bank = this->bank();
@@ -2368,6 +2638,7 @@ class TracedSynth
     if (times_) times_->reset(inst);
     bank.reset(lanes);
     if (pubBank_) pubBank_->reset(inst);
+    if (ibank_) ibank_->reset(inst);
   }
 
   // getPublishedSignals()[name]->readLatest(dest, frames) of every instrument in one call (MLSignalProcessor.cpp:19-28):

@@ -146,6 +146,8 @@ def lib() -> ctypes.CDLL:
                                                 ctypes.c_int]
     L.mlb_synth_process_context_host.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int, _vp, _vp,
                                                  ctypes.c_int, _vp, _vp, _vp, ctypes.c_int]
+    L.mlb_synth_process_instrument_host.argtypes = [_vp] * 10 + [ctypes.c_int, _vp, _vp, ctypes.c_int, _vp,
+                                                                 ctypes.c_int]
     L.mlb_graph_process_host.argtypes = [_vp, _vp, _vp, _vp, ctypes.c_int]
     L.mlb_graph_last_kernel_ms.argtypes = [_vp, _vp]
     L.mlb_graph_last_host_slices.argtypes = [_vp]
@@ -545,6 +547,33 @@ class VoiceGraph(_Handle):
             _ptr(toff), tr.ctypes.data if tr is not None and tr.size else None, 0 if tr is None else int(tr.size),
             _ptr(out), _ptr(mix), _ptr(bus), T))
         return bus if buses is not None else (out, mix)
+
+    def process_instrument_host(self, instrument: "VoiceGraph", routers: "RouterBank", bank: "VoiceBank",
+                                buses: "Buses", offsets: np.ndarray, events: np.ndarray,
+                                controllers: Optional["ControllerBank"] = None, times: Optional["ProcessTimeBank"] = None,
+                                time_offsets: Optional[np.ndarray] = None, transports: Optional[np.ndarray] = None,
+                                bus: Optional[np.ndarray] = None) -> np.ndarray:
+        """process_context_host with buses, then ``instrument``, a graph over the buses' instruments, on the bus sums,
+        the controller planes and the beat phase (mlb_synth_process_instrument_host).  Returns (or writes into
+        ``bus``) its outputs [T][instrument outputs][G][64]."""
+        name = "process_instrument_host"
+        off, T = _offset_table(name, offsets, routers.n_instruments)
+        bus = _out_array(name, "bus", bus, (T, instrument.spec.n_out, buses.n_buses, BLOCK))
+        ev = np.ascontiguousarray(events, EVENT_DTYPE)
+        toff = tr = None
+        if times is not None:
+            if time_offsets is None or transports is None:
+                raise ValueError(f"{name}: a process-time bank needs time_offsets and transports")
+            toff = np.ascontiguousarray(time_offsets, np.int32)
+            if toff.shape != off.shape:
+                raise ValueError(f"{name}: time_offsets must be {off.shape}, got {toff.shape}")
+            tr = np.ascontiguousarray(transports, TRANSPORT_DTYPE)
+        _check(lib().mlb_synth_process_instrument_host(
+            routers._h, bank._h, controllers._h if controllers else None, times._h if times else None, self._h,
+            buses._h, None, instrument._h, off.ctypes.data, ev.ctypes.data if ev.size else None, int(ev.size),
+            _ptr(toff), tr.ctypes.data if tr is not None and tr.size else None, 0 if tr is None else int(tr.size),
+            _ptr(bus), T))
+        return bus
 
     def process_device(self, inp, out, mix, n_blocks: int, stream: int = 0) -> None:
         """Device pointers (torch tensors / ints); asynchronous on ``stream`` (cudaStream_t)."""

@@ -34,16 +34,9 @@ MLB_DEV float2 ld_stream_f2(const float2* p)
   return r;
 }
 
-__global__ void __launch_bounds__(32 * kBusWarps) bus_sum_kernel(BusArgs a)
+// ((+0 + x[0]) + x[1]) + ... over `count` voice rows 64 floats apart, from src (this lane's two columns)
+MLB_DEV float2 sum_voices(const float2* src, int count)
 {
-  const long long w = (long long)blockIdx.x * kBusWarps + (threadIdx.x >> 5);
-  if (w >= a.n_items) return;
-  const int lane = threadIdx.x & 31;
-  const int g = (int)(w % a.G);
-  const long long tp = w / a.G;  // t * P + p
-  const long long row = tp + (tp / a.P) * (a.stride - a.P);  // t * stride + p
-  const int first = __ldg(a.first + g), count = __ldg(a.count + g);
-  const float2* src = reinterpret_cast<const float2*>(a.rows + ((size_t)row * a.V + first) * MLB_BLOCK) + lane;
   float2 acc = make_float2(0.f, 0.f);
   for (int i = 0; i < count; i += kBusAhead)
   {
@@ -59,7 +52,55 @@ __global__ void __launch_bounds__(32 * kBusWarps) bus_sum_kernel(BusArgs a)
         acc.y = __fadd_rn(acc.y, x[u].y);
       }
   }
-  reinterpret_cast<float2*>(a.bus + (size_t)w * MLB_BLOCK)[lane] = acc;
+  return acc;
+}
+
+__global__ void __launch_bounds__(32 * kBusWarps) bus_sum_kernel(BusArgs a)
+{
+  const long long w = (long long)blockIdx.x * kBusWarps + (threadIdx.x >> 5);
+  if (w >= a.n_items) return;
+  const int lane = threadIdx.x & 31;
+  const int g = (int)(w % a.G);
+  const long long tp = w / a.G;  // t * P + p
+  const long long row = tp + (tp / a.P) * (a.stride - a.P);  // t * stride + p
+  const int first = __ldg(a.first + g), count = __ldg(a.count + g);
+  const float2* src = reinterpret_cast<const float2*>(a.rows + ((size_t)row * a.V + first) * MLB_BLOCK) + lane;
+  reinterpret_cast<float2*>(a.bus + (size_t)w * MLB_BLOCK)[lane] = sum_voices(src, count);
+}
+
+// The input planes of an instrument graph (Synth::processVector overridden around the base call):
+// in [T][P + C][G][64], planes 0..P-1 the bus sums exactly as bus_sum_kernel makes them, planes P..P+C-1 bit copies of
+// planes plane0..plane0+C-1 of the voice planes at the bus's first voice (the controllers and the beat phase, which
+// every voice of an instrument holds alike).  A copy is a move, not +0 + x, which would turn -0 into +0.
+struct InstrumentInputArgs
+{
+  BusArgs bus;          // bus.bus unused; bus.P: the bus planes
+  const float* voice;   // [T][voice_stride][V][64]
+  float* in;            // [T][P + C][G][64]
+  int voice_stride, plane0, C;
+  long long n_items;    // T * (P + C) * G
+};
+
+__global__ void __launch_bounds__(32 * kBusWarps) instrument_inputs_kernel(InstrumentInputArgs a)
+{
+  const long long w = (long long)blockIdx.x * kBusWarps + (threadIdx.x >> 5);
+  if (w >= a.n_items) return;
+  const int lane = threadIdx.x & 31;
+  const BusArgs& b = a.bus;
+  const int g = (int)(w % b.G), NI = b.P + a.C;
+  const long long tq = w / b.G;
+  const long long t = tq / NI;
+  const int q = (int)(tq - t * NI);
+  const int first = __ldg(b.first + g);
+  float2 y;
+  if (q < b.P)
+    y = sum_voices(reinterpret_cast<const float2*>(b.rows + (((size_t)t * b.stride + q) * b.V + first) * MLB_BLOCK) + lane,
+                   __ldg(b.count + g));
+  else
+    y = ld_stream_f2(reinterpret_cast<const float2*>(
+                         a.voice + (((size_t)t * a.voice_stride + a.plane0 + (q - b.P)) * b.V + first) * MLB_BLOCK) +
+                     lane);
+  reinterpret_cast<float2*>(a.in + (size_t)w * MLB_BLOCK)[lane] = y;
 }
 
 }  // namespace mlb

@@ -2615,6 +2615,7 @@ struct SynthCall
   int n_transports = 0;
   mlb_buses* b = nullptr;
   mlb_published* p = nullptr;  // with b: K14 after the bus sum, over the graph's last mlb_published_planes outputs
+  mlb_graph* gi = nullptr;     // with b: the instrument graph over b's G buses, on the bus sums, controllers and beat phase
   float *out = nullptr, *mix = nullptr, *bus = nullptr;
   int run() const;  // the driver
 };
@@ -2635,6 +2636,7 @@ struct mlb_buses
 {
   LiveCount live;
   int V = 0, G = 0;
+  int empty = 0;            // buses of no voice
   DevBuf<int32_t> d_table;  // [2][G]: first voice, voice count
   DevBuf<float> d_out;      // bus rows of mlb_synth_process_buses_host, [T][n_out][G][64]
 };
@@ -2662,6 +2664,7 @@ extern "C" int mlb_buses_create(int n_voices, int n_buses, const int32_t* first_
   std::unique_ptr<mlb_buses> b(new mlb_buses);
   b->live.arm();
   b->V = n_voices, b->G = n_buses;
+  for (int g = 0; g < n_buses; ++g) b->empty += voice_count[g] == 0;
   const size_t bytes = (size_t)n_buses * sizeof(int32_t);
   MLB_TRY(b->d_table.alloc(2 * bytes, "bus layout"));
   if (cudaMemcpy(b->d_table.get(), first_voice, bytes, cudaMemcpyHostToDevice) != cudaSuccess ||
@@ -2682,6 +2685,25 @@ static int bus_sum(mlb_buses* b, const float* rows_dev, float* bus_dev, int n_pl
   const long long grid = (a.n_items + kBusWarps - 1) / kBusWarps;
   if (grid > 0x7FFFFFFFLL) return fail(MLB_ERR_INVALID, "%lld bus rows exceed one launch", a.n_items);
   bus_sum_kernel<<<(unsigned)grid, 32 * kBusWarps, 0, (cudaStream_t)stream>>>(a);
+  ++g_launches;
+  CU_CHECK(cudaGetLastError());
+  return MLB_OK;
+}
+
+// The instrument graph's input planes [T][n_planes + n_copy][G][64]: the bus sums of rows [T][stride][V][64] planes
+// 0..n_planes-1, then planes plane0..plane0+n_copy-1 of voice [T][voice_stride][V][64] copied from each bus's first voice
+static int instrument_inputs(mlb_buses* b, const float* rows_dev, int n_planes, int stride, const float* voice_dev,
+                             int voice_stride, int plane0, int n_copy, float* in_dev, int n_blocks, cudaStream_t stream)
+{
+  InstrumentInputArgs a;
+  a.bus.rows = rows_dev, a.bus.bus = nullptr, a.bus.first = b->d_table.get(), a.bus.count = b->d_table.get() + b->G;
+  a.bus.V = b->V, a.bus.G = b->G, a.bus.P = n_planes, a.bus.stride = stride;
+  a.voice = voice_dev, a.in = in_dev, a.voice_stride = voice_stride, a.plane0 = plane0, a.C = n_copy;
+  a.n_items = (long long)n_blocks * (n_planes + n_copy) * b->G;
+  a.bus.n_items = a.n_items;
+  const long long grid = (a.n_items + kBusWarps - 1) / kBusWarps;
+  if (grid > 0x7FFFFFFFLL) return fail(MLB_ERR_INVALID, "%lld instrument input rows exceed one launch", a.n_items);
+  instrument_inputs_kernel<<<(unsigned)grid, 32 * kBusWarps, 0, stream>>>(a);
   ++g_launches;
   CU_CHECK(cudaGetLastError());
   return MLB_OK;
@@ -3509,7 +3531,7 @@ extern "C" int mlb_published_read_host(mlb_published* p, int signal, int mode, i
 }
 
 static int synth_routed(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb, mlb_process_time* pt, mlb_graph* g,
-                        mlb_buses* b, mlb_published* p, const int32_t* offsets_host, const mlb_event* events_host, int n_events,
+                        mlb_buses* b, mlb_published* p, mlb_graph* gi, const int32_t* offsets_host, const mlb_event* events_host, int n_events,
                         const int32_t* time_offsets_host, const mlb_transport* transports_host, int n_transports,
                         float* out_host, float* mix_host, float* bus_host, int n_blocks)
 {
@@ -3546,6 +3568,20 @@ static int synth_routed(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb, mlb
   if (pt && !time_offsets_host) return fail(MLB_ERR_INVALID, "null transport offsets");
   if (pt && (n_transports < 0 || (n_transports > 0 && !transports_host)))
     return fail(MLB_ERR_INVALID, "%d transport updates at %p", n_transports, (const void*)transports_host);
+  if (gi)
+  {
+    // its input planes: the P bus planes (the graph's audio outputs), then the C controller planes and the beat phase
+    const int P = (int)g->outs.size() - (p ? p->Q : 0), NI = P + (cb ? cb->C : 0) + (pt ? 1 : 0);
+    if (!b) return fail(MLB_ERR_INVALID, "an instrument graph needs buses");
+    if (gi->V != r->G) return fail(MLB_ERR_INVALID, "instrument graph has %d lanes, router bank %d instruments", gi->V, r->G);
+    if (b->G != r->G) return fail(MLB_ERR_INVALID, "buses have %d instruments, router bank %d", b->G, r->G);
+    if (b->empty) return fail(MLB_ERR_INVALID, "%d buses have no voice; an instrument graph reads each bus's first voice", b->empty);
+    for (const mlb_node& n : gi->nodes)
+      if (n.op == MLB_OP_INPUT && (n.iarg < 0 || n.iarg >= NI))
+        return fail(MLB_ERR_INVALID, "instrument graph INPUT plane %d is not a bus plane (0..%d), controller plane or the "
+                    "beat-phase plane (%d planes in all)", n.iarg, P - 1, NI);
+    MLB_TRY(graph_check(gi, n_blocks, NI, offsets_host, true));
+  }
   int n_changes = 0;
   MLB_TRY(routers_check(r, offsets_host, events_host, n_events, n_blocks, &n_changes));
   if (pt) MLB_TRY(check_offsets(time_offsets_host, pt->G, n_transports, n_blocks, "transport", "updates"));
@@ -3553,6 +3589,7 @@ static int synth_routed(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb, mlb
   c.r = r, c.offsets = offsets_host, c.events = events_host, c.n_events = n_events, c.n_changes = n_changes, c.cb = cb;
   c.pt = pt, c.time_offsets = time_offsets_host, c.transports = transports_host, c.n_transports = n_transports;
   c.p = p && p->Q ? p : nullptr;
+  c.gi = gi;
   return c.run();
 }
 
@@ -3569,11 +3606,14 @@ int SynthCall::run() const
   MLB_TRY(ensure_init());
   const size_t V = (size_t)g->V, T = (size_t)n_blocks, n_rows = g->outs.size();
   const size_t n_out = n_rows - (p ? (size_t)p->Q : 0);  // the audio planes; the published planes follow them
+  const size_t n_bus = gi ? gi->outs.size() : n_out;      // bus rows per block and instrument: what comes back
+  const int n_copy = n_planes - MLB_VOICE_ROWS;            // the instrument graph's controller and beat-phase planes
   const size_t G1 = (size_t)(r ? r->G : cb ? cb->G : 0) + 1;  // pt->G is r->G
   const int Tc = synth_chunk_blocks(g, n_blocks, n_planes);
   if (out) MLB_TRY(g->d_out.ensure(T * n_out * V * MLB_BLOCK * 4, "staging"));
   if (b) MLB_TRY(g->d_out.ensure((size_t)Tc * n_rows * V * MLB_BLOCK * 4, "staging"));
-  if (b) MLB_TRY(b->d_out.ensure(T * n_out * b->G * MLB_BLOCK * 4, "staging"));
+  if (b) MLB_TRY(b->d_out.ensure(T * n_bus * b->G * MLB_BLOCK * 4, "staging"));
+  if (gi) MLB_TRY(gi->d_in.ensure((size_t)Tc * (n_out + n_copy) * b->G * MLB_BLOCK * 4, "staging"));
   if (mix) MLB_TRY(g->d_mix.ensure(T * n_out * MLB_BLOCK * 4, "staging"));
   if (r)
   {
@@ -3592,7 +3632,7 @@ int SynthCall::run() const
   if (pt) MLB_TRY(pt->d_off.ensure(T * G1 * 4, "staging"));
   if (pt) MLB_TRY(pt->d_tr.ensure(std::max(n_transports, 1) * sizeof(mlb_transport), "staging"));
   const size_t row_floats = n_out * V * MLB_BLOCK;             // output rows per block
-  const size_t bus_floats = b ? n_out * b->G * MLB_BLOCK : 0;  // bus rows per block
+  const size_t bus_floats = b ? n_bus * b->G * MLB_BLOCK : 0;  // bus rows per block
   float* down_dev = b ? b->d_out.get() : g->d_out.get();
   float* down_host = b ? bus : out;
   const size_t down_floats = b ? bus_floats : row_floats;
@@ -3628,8 +3668,15 @@ int SynthCall::run() const
           if (b)
           {
             MLB_TRY(graph_process(g, vb->d_out.get(), n_planes, g->d_out.get(), nullptr, t1 - t0, s));
-            MLB_TRY(bus_sum(b, g->d_out.get(), b->d_out.get() + t0 * bus_floats, (int)n_out, (int)n_rows, t1 - t0, s));
-            return p ? mlb_published_process_device(p, g->d_out.get(), (int)n_out, (int)n_rows, t1 - t0, s) : MLB_OK;
+            if (gi)
+              MLB_TRY(instrument_inputs(b, g->d_out.get(), (int)n_out, (int)n_rows, vb->d_out.get(), n_planes,
+                                        MLB_VOICE_ROWS, n_copy, gi->d_in.get(), t1 - t0, s));
+            else
+              MLB_TRY(bus_sum(b, g->d_out.get(), b->d_out.get() + t0 * bus_floats, (int)n_out, (int)n_rows, t1 - t0, s));
+            if (p) MLB_TRY(mlb_published_process_device(p, g->d_out.get(), (int)n_out, (int)n_rows, t1 - t0, s));
+            return gi ? graph_process(gi, gi->d_in.get(), (int)n_out + n_copy, b->d_out.get() + t0 * bus_floats, nullptr,
+                                      t1 - t0, s)
+                      : MLB_OK;
           }
           return graph_process(g, vb->d_out.get(), n_planes, out ? g->d_out.get() + t0 * row_floats : nullptr,
                                mix ? g->d_mix.get() + t0 * n_out * MLB_BLOCK : nullptr, t1 - t0, s);
@@ -3652,8 +3699,8 @@ extern "C" int mlb_synth_process_routed_host(mlb_routers* r, mlb_voices* vb, mlb
                                              int n_events, float* out_host, float* mix_host, float* bus_host,
                                              int n_blocks)
 {
-  return synth_routed(r, vb, cb, nullptr, g, b, nullptr, offsets_host, events_host, n_events, nullptr, nullptr, 0, out_host,
-                      mix_host, bus_host, n_blocks);
+  return synth_routed(r, vb, cb, nullptr, g, b, nullptr, nullptr, offsets_host, events_host, n_events, nullptr, nullptr,
+                      0, out_host, mix_host, bus_host, n_blocks);
 }
 
 extern "C" int mlb_synth_process_context_host(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb,
@@ -3663,7 +3710,7 @@ extern "C" int mlb_synth_process_context_host(mlb_routers* r, mlb_voices* vb, ml
                                               int n_transports, float* out_host, float* mix_host, float* bus_host,
                                               int n_blocks)
 {
-  return synth_routed(r, vb, cb, pt, g, b, nullptr, offsets_host, events_host, n_events, time_offsets_host,
+  return synth_routed(r, vb, cb, pt, g, b, nullptr, nullptr, offsets_host, events_host, n_events, time_offsets_host,
                       transports_host, n_transports, out_host, mix_host, bus_host, n_blocks);
 }
 
@@ -3674,7 +3721,19 @@ extern "C" int mlb_synth_process_published_host(mlb_routers* r, mlb_voices* vb, 
                                                 int n_transports, float* bus_host, int n_blocks)
 {
   if (!p) return fail(MLB_ERR_INVALID, "null published bank");
-  return synth_routed(r, vb, cb, pt, g, b, p, offsets_host, events_host, n_events, time_offsets_host, transports_host,
+  return synth_routed(r, vb, cb, pt, g, b, p, nullptr, offsets_host, events_host, n_events, time_offsets_host,
+                      transports_host, n_transports, nullptr, nullptr, bus_host, n_blocks);
+}
+
+extern "C" int mlb_synth_process_instrument_host(mlb_routers* r, mlb_voices* vb, mlb_controllers* cb,
+                                                 mlb_process_time* pt, mlb_graph* g, mlb_buses* b, mlb_published* p,
+                                                 mlb_graph* gi, const int32_t* offsets_host, const mlb_event* events_host,
+                                                 int n_events, const int32_t* time_offsets_host,
+                                                 const mlb_transport* transports_host, int n_transports, float* bus_host,
+                                                 int n_blocks)
+{
+  if (!gi) return fail(MLB_ERR_INVALID, "null instrument graph");
+  return synth_routed(r, vb, cb, pt, g, b, p, gi, offsets_host, events_host, n_events, time_offsets_host, transports_host,
                       n_transports, nullptr, nullptr, bus_host, n_blocks);
 }
 
